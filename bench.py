@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Headline benchmark (driver contract): samples/sec of the launched DDP training job.
 
-    python bench.py --gpus N --steps K --warmup W [--model gpt2|bert|resnet50|mnist]
+    python bench.py --gpus N --steps K --warmup W [--model gpt2|bert|resnet50|mnist] [--dump-outputs DIR]
 
 * ``value``  -- device-timed (CUDA events, max over ranks) whole-job samples/sec of the flagship
   training step (GPT-2 small, seq 1024, bf16, per-GPU batch 16 = weak scaling) run by the ranks the
@@ -15,6 +15,10 @@
   code and no cluster to run against here: prints ``{"impl": "reference", "unavailable": ...}``.
 
 BASELINE.json publishes no numbers (``published: {}``), so ``vs_baseline`` is null.
+
+``--dump-outputs DIR``: after the timed steps, rank 0 writes what they computed (the per-step losses and a seeded sample
+of the updated fp32 master weights, ``runtime.worker.dump_outputs``) as ``DIR/*.npy``.  Inputs and initial weights are
+seeded, so two builds run with the same arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -40,7 +44,7 @@ MODEL_DEFAULTS = {
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
@@ -101,7 +105,7 @@ class ClockSampler:
                 "scope": scope}
 
 
-def worker_args(a, result_path=""):
+def worker_args(a, result_path="", dump_dir=""):
     from trainingjob_operator_b200.runtime import worker
 
     d = MODEL_DEFAULTS[a.model]
@@ -111,6 +115,8 @@ def worker_args(a, result_path=""):
         argv.append("--no-graph")
     if result_path:
         argv += ["--result", result_path]
+    if dump_dir:
+        argv += ["--dump-outputs", dump_dir]
     return worker.parse_args(argv), argv
 
 
@@ -124,7 +130,7 @@ def run_device_timed(a):
     os.environ.setdefault("MASTER_PORT", "29511")
     os.environ.pop("AITJ_MASTER", None)
     rank = int(os.environ["RANK"])
-    wa, _ = worker_args(a)
+    wa, _ = worker_args(a, dump_dir=a.dump_outputs)
     sampler = ClockSampler() if rank == 0 else None
     if sampler:
         sampler.start()
@@ -242,11 +248,13 @@ def main():
     ap.add_argument("--model", default="gpt2", choices=sorted(MODEL_DEFAULTS))
     ap.add_argument("--batch", type=int, default=0, help="per-GPU batch (default per model)")
     ap.add_argument("--seq", type=int, default=0)
-    ap.add_argument("--gemm", default="tcgen05", choices=["tcgen05", "cublas"])
+    ap.add_argument("--gemm", default="wgmma", choices=["wgmma", "cublas"])
     ap.add_argument("--no-graph", action="store_true")
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-warm-pool", action="store_true", help="e2e arm: cold worker start instead of the agent's warm pool")
     ap.add_argument("--e2e-timeout", type=float, default=900.0)
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="write what the timed steps computed (losses, seeded sample of the updated weights) to DIR/*.npy")
     a = ap.parse_args()
     a.warmup = max(3, a.warmup)
 
@@ -318,7 +326,7 @@ def main():
                    "optimizer": "AdamW (fused flat sweep, fp32 master + bf16 compute copy), grad-clip 1.0",
                    "cuda_graph": res.get("cuda_graph"), "graph_error": res.get("graph_error"),
                    "allreduce": res.get("allreduce"),
-                   "l2": "working set (params+activations >> 126 MB L2) exceeds L2; inputs change every step",
+                   "l2": "working set (params+activations >> 50 MB L2) exceeds L2; inputs change every step",
                    "loss_first": res.get("loss_first"), "loss_last": res.get("loss_last")},
         "clocks": clocks,
         "e2e": e2e,
@@ -326,8 +334,8 @@ def main():
         "launches_per_step": res.get("launches_per_step"),
         "tokens_per_sec": res["samples_per_sec"] * (res["describe"].get("seq_len") or 1),
         "model_tflops": flops / (ms / 1e3) / 1e12 if flops else None,
-        "mfu_of_measured_bf16_sustained": (flops / (ms / 1e3) / 1e12 / (peaks.get("bf16_tflops_sustained", 1451.7) * a.gpus))
-        if flops else None,
+        "mfu_of_measured_bf16_sustained": (flops / (ms / 1e3) / 1e12 / (peaks["bf16_tflops_sustained"] * a.gpus))
+        if flops and "bf16_tflops_sustained" in peaks else None,
     }
     print(json.dumps(line), flush=True)
     return 0

@@ -7,7 +7,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: test needs a CUDA device (run on a B200 via gpurun)")
+    config.addinivalue_line("markers", "gpu: test needs a CUDA device (an H100)")
     config.addinivalue_line("markers", "gpu2: GPU test that needs at least two devices (also marked gpu; skipped on a 1-GPU box)")
     config.addinivalue_line("markers", "slow: multi-process / long-running CPU test")
 

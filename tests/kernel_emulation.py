@@ -1,7 +1,7 @@
 """Plain-PyTorch stand-ins for the entry points of ``trainingjob_operator_b200.ops.functional`` -- TEST ONLY.
 
 The engines (``models/gpt2.py``, ``models/bert.py``), the trainer and the worker adapters only run on a GPU box, where
-they call hand-written sm_100a kernels; nothing of that can execute in the build container.  ``install()`` replaces the
+they call hand-written sm_90a kernels; nothing of that can execute without a GPU.  ``install()`` replaces the
 kernel entry points by functions with the same contracts (same arguments, same in-place outputs, same accumulate /
 overwrite rules, bf16 storage with fp32 math) so that the *control flow around the kernels* -- buffer rotation, which
 gradient goes where, bucket hooks, optimizer arguments, the per-GEMM kernel table, the side-stream bookkeeping -- runs
@@ -125,11 +125,11 @@ def _gelu_grad(x: torch.Tensor) -> torch.Tensor:
 
 
 def num_sms() -> int:
-    return 148
+    return 132
 
 
 def gemm(a, b, out, *, a_mn=False, b_mn=False, bias=None, residual=None, aux=None, gelu=False, dgelu=False,
-         save_pre=False, accumulate=False, split_k=1, block_n=0, max_ctas=0, colsum=None, _debug_skip_epilogue=False):
+         save_pre=False, accumulate=False, split_k=1, block_n=0, max_ctas=0, colsum=None):
     CALLS["n"] += 1
     CALLS["gemm_block_n"].append(block_n)
     assert a.dtype == torch.bfloat16 and b.dtype == torch.bfloat16

@@ -6,7 +6,9 @@ import os
 import subprocess
 import sys
 import textwrap
+import types
 
+import numpy as np
 import pytest
 import torch
 
@@ -27,7 +29,7 @@ def gpt2_pair(monkeypatch, env=None, seed=3):
         monkeypatch.setenv(k, v)
     cfg = GPT2Config(vocab_size=1000, n_layer=2, n_head=4, n_embd=256, block_size=128, name="t")
     B, T = 2, 128
-    eng = GPT2Engine(cfg, B, T, "cpu", seed=seed, gemm_backend="tcgen05")
+    eng = GPT2Engine(cfg, B, T, "cpu", seed=seed, gemm_backend="wgmma")
     g = torch.Generator().manual_seed(9)
     for s_ in eng.params.specs:               # biases / LayerNorm gains away from their symmetric initial values
         if len(s_.shape) == 1:
@@ -45,8 +47,8 @@ GPT2_GRADS = ("wte", "wpe", "h0.qkv_w", "h0.qkv_b", "h0.proj_w", "h0.proj_b", "h
               "h0.fc2_b", "h0.ln1_w", "h0.ln1_b", "h1.ln2_w", "h1.ln2_b", "h1.fc2_w", "h1.qkv_w", "lnf_w", "lnf_b")
 
 
-# (AITJ_ATTN=tcgen05 with the library backward calls a cuDNN-only aten op: that combination exists on the GPU only)
-@pytest.mark.parametrize("env", [{}, {"AITJ_ATTN": "tcgen05", "AITJ_ATTN_BWD": "tcgen05"},
+# (AITJ_ATTN=wgmma with the library backward calls a cuDNN-only aten op: that combination exists on the GPU only)
+@pytest.mark.parametrize("env", [{}, {"AITJ_ATTN": "wgmma", "AITJ_ATTN_BWD": "wgmma"},
                                  {"AITJ_GEMM_CFG": "fwd:768x256=256,dgrad:256x768=128,wgrad:1024x256=512/4"},
                                  {"AITJ_GEMM_PAIR": "0"}],
                          ids=["default", "attn-fwd-bwd", "gemm-table", "no-pair"])
@@ -56,7 +58,7 @@ def test_gpt2_engine_control_flow_matches_the_reference_model(monkeypatch, env):
     shows as an O(1) error; bf16 storage of activations costs ~1e-2)."""
     cfg, eng, ref, tok, tgt = gpt2_pair(monkeypatch, env)
     if env.get("AITJ_ATTN"):
-        assert eng.attn_impl == "tcgen05" and eng.attn_bwd_impl == env.get("AITJ_ATTN_BWD", "cudnn")
+        assert eng.attn_impl == "wgmma" and eng.attn_bwd_impl == env.get("AITJ_ATTN_BWD", "cudnn")
     eng.params.g32.zero_()
     eng.forward()
     eng.backward()
@@ -187,7 +189,7 @@ from trainingjob_operator_b200.runtime.trainer import EngineTrainer
 rank, world = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"])
 dist.init_process_group("gloo", rank=rank, world_size=world)
 cfg = GPT2Config(vocab_size=1000, n_layer=2, n_head=4, n_embd=256, block_size=128, name="t")
-eng = GPT2Engine(cfg, 2, 128, "cpu", seed=3, gemm_backend="tcgen05")
+eng = GPT2Engine(cfg, 2, 128, "cpu", seed=3, gemm_backend="wgmma")
 tr = EngineTrainer(eng, lr=1e-3, use_graph=False, allreduce="nccl")
 assert tr.reducer is not None and tr.segmented and eng.segment_join is True
 g = torch.Generator().manual_seed(100 + rank)          # every rank its own data
@@ -592,7 +594,7 @@ def test_stall_exit_makes_a_pod_scope_restart_whole_again_in_seconds(tmp_path):
             time.sleep(0.5)
 
 
-def test_owner_sharded_data_parallel_equals_one_replica_on_the_joint_batch(monkeypatch):
+def test_owner_sharded_data_parallel_equals_one_replica_on_the_joint_batch(monkeypatch, tmp_path):
     """The default multi-GPU algorithm (``AITJ_ALLREDUCE=rs``) with its peer-memory kernels emulated: two "ranks" (threads
     with a real barrier where the device-side barriers are) each see half of a batch; gradient producers add every
     piece into the copy of the rank that OWNS it, the owner clips on the exchanged partial norms and runs AdamW on its
@@ -617,7 +619,7 @@ def test_owner_sharded_data_parallel_equals_one_replica_on_the_joint_batch(monke
         eng.params.refresh_compute_copy()
 
     # ---- reference: one replica, the joint batch
-    ref = GPT2Engine(cfg, N * B, T, "cpu", seed=3, gemm_backend="tcgen05")
+    ref = GPT2Engine(cfg, N * B, T, "cpu", seed=3, gemm_backend="wgmma")
     perturb(ref)
     for step in range(STEPS):
         ref.tok.copy_(toks[step].view(-1))
@@ -631,7 +633,7 @@ def test_owner_sharded_data_parallel_equals_one_replica_on_the_joint_batch(monke
     ke._CURRENT["world"] = fw
     engs = []
     for r in range(N):
-        e = GPT2Engine(cfg, B, T, "cpu", seed=3, gemm_backend="tcgen05")
+        e = GPT2Engine(cfg, B, T, "cpu", seed=3, gemm_backend="wgmma")
         perturb(e)
         fw.attach(e.params)
         engs.append(e)
@@ -679,6 +681,45 @@ def test_owner_sharded_data_parallel_equals_one_replica_on_the_joint_batch(monke
     joint = float(ref.sumsq) ** 0.5
     sharded = float(fw.shards[1].parts[:N].sum()) ** 0.5 / N
     assert abs(sharded - joint) < 2e-3 * joint, (sharded, joint)
+    # bench.py --dump-outputs: every rank gathers the shards (EngineAdapter.prepare_state, a collective -- broadcasts
+    # emulated between the two threads), then rank 0 writes its fp32 master weights: they must be the joint-batch
+    # replica's everywhere, not only in rank 0's own shard
+    from trainingjob_operator_b200.runtime import worker as W
+
+    assert rel(engs[0].params.p32, ref.params.p32) > 1e-2               # before the gather: rank 1's shard is stale
+    sync = threading.Barrier(N)
+    box, me = {}, threading.local()
+
+    def fake_broadcast(t, src):
+        me.calls = getattr(me, "calls", 0) + 1
+        if me.rank == src:
+            box[me.calls] = t.clone()
+        sync.wait()
+        if me.rank != src:
+            t.copy_(box[me.calls])
+        sync.wait()
+
+    real = (W.dist.is_initialized, W.dist.broadcast)
+    monkeypatch.setattr(W.dist, "is_initialized", lambda: True)
+    monkeypatch.setattr(W.dist, "broadcast", fake_broadcast)
+    adapters = [types.SimpleNamespace(engine=e, state_tensors=e.params.state_tensors) for e in engs]
+
+    def gather(r):
+        me.rank = r
+        W.EngineAdapter.prepare_state(adapters[r])
+
+    threads = [threading.Thread(target=gather, args=(r,)) for r in range(N)]
+    for t in threads:
+        t.start()
+    for t in threads:
+        t.join(120)
+    W.dump_outputs(str(tmp_path), adapters[0], [1.0, 2.0])
+    dumped = torch.from_numpy(np.load(tmp_path / "weights_sample.npy"))
+    assert dumped.numel() == ref.params.p32.numel()
+    assert rel(dumped, ref.params.p32) < 2e-4
+    assert np.load(tmp_path / "losses.npy").tolist() == [1.0, 2.0]
+    monkeypatch.setattr(W.dist, "is_initialized", real[0])
+    monkeypatch.setattr(W.dist, "broadcast", real[1])
     # leaving the sharded mode (world shrank to one rank, re-bind after a re-rendezvous): private buffers again, the bf16
     # parameters kept, gradients plain local tensors
     P = engs[0].params

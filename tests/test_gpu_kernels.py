@@ -1,4 +1,4 @@
-"""GPU numerics tests: each hand-written sm_100a kernel vs. a plain fp32 PyTorch reference.
+"""GPU numerics tests: each hand-written sm_90a kernel vs. a plain fp32 PyTorch reference.
 
 Cases run in their own process (``ops.selfcheck``) so one trapping kernel cannot poison the
 CUDA context of the others.

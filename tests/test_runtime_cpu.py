@@ -479,7 +479,7 @@ def test_nn_module_workers_step_on_cpu(name, batch, params):
 
     from trainingjob_operator_b200.runtime import worker as W
 
-    args = types.SimpleNamespace(seed=0, lr=1e-3, no_graph=True, gemm="tcgen05")
+    args = types.SimpleNamespace(seed=0, lr=1e-3, no_graph=True, gemm="wgmma")
     ad = W.TorchAdapter(name, batch, args, torch.device("cpu"))
     ad.bind(None)
     assert sum(p.numel() for p in ad.module.parameters()) == params

@@ -17,8 +17,13 @@ try:
     PEAKS = json.load(open(os.path.join(os.path.dirname(__file__), "..", "MEASURED_PEAKS.json")))
 except Exception:
     pass
-PEAK_TF = PEAKS.get("bf16_tflops", 1590.0)
-PEAK_BW = PEAKS.get("hbm_gbs", 6650.0)
+# shares of a peak are only reported against peaks measured on the same card (MEASURED_PEAKS.json); null otherwise
+PEAK_TF = PEAKS.get("bf16_tflops")
+PEAK_BW = PEAKS.get("hbm_gbs")
+
+
+def frac(rate, peak):
+    return rate / peak if peak else None
 
 _flush = None
 
@@ -71,12 +76,12 @@ def main():
         flops = 2.0 * m * n * k
         for bn in (1024, 512, 256):
             med, best = timeit(lambda: F.gemm(a, b, out, a_mn=a_mn, b_mn=b_mn, block_n=bn))
-            rows.append({"kernel": f"tcgen05 {name} bn={bn}", "M": m, "N": n, "K": k, "ms_med": med, "ms_best": best,
-                         "tflops": flops / med / 1e9, "frac_of_measured_peak": flops / med / 1e9 / PEAK_TF})
+            rows.append({"kernel": f"wgmma {name} bn={bn}", "M": m, "N": n, "K": k, "ms_med": med, "ms_best": best,
+                         "tflops": flops / med / 1e9, "frac_of_measured_peak": frac(flops / med / 1e9, PEAK_TF)})
         bt = b if b_mn else b.t()
         med, best = timeit(lambda: torch.matmul(a, bt, out=out))
         rows.append({"kernel": f"cublas  {name}", "M": m, "N": n, "K": k, "ms_med": med, "ms_best": best,
-                     "tflops": flops / med / 1e9, "frac_of_measured_peak": flops / med / 1e9 / PEAK_TF})
+                     "tflops": flops / med / 1e9, "frac_of_measured_peak": frac(flops / med / 1e9, PEAK_TF)})
     # wgrad (split-K, fp32 red.add)
     for name, nout, kin in ([] if mem_only else [("qkv wgrad", 3 * C, C), ("fc wgrad", 4 * C, C), ("fc2 wgrad", C, 4 * C),
                                                  ("proj wgrad", C, C), ("lm_head wgrad", 50304, C)]):
@@ -88,16 +93,16 @@ def main():
         for bn, tag in ((1024, "quad"), (512, "2cta"), (0, "1cta")):
             skk = F.auto_split_k(nout, kin, M, 256) * (2 if bn >= 512 else 1)
             med, best = timeit(lambda: F.gemm(dy, x, dw, a_mn=True, b_mn=True, accumulate=True, split_k=skk, block_n=bn))
-            rows.append({"kernel": f"tcgen05 {name} {tag} sk={skk}", "M": nout, "N": kin, "K": M, "ms_med": med,
+            rows.append({"kernel": f"wgmma {name} {tag} sk={skk}", "M": nout, "N": kin, "K": M, "ms_med": med,
                          "ms_best": best, "tflops": flops / med / 1e9,
-                         "frac_of_measured_peak": flops / med / 1e9 / PEAK_TF})
+                         "frac_of_measured_peak": frac(flops / med / 1e9, PEAK_TF)})
         med, best = timeit(lambda: F.gemm(dy, x, dw, a_mn=True, b_mn=True, accumulate=True, split_k=sk))
-        rows.append({"kernel": f"tcgen05 {name} sk={sk}", "M": nout, "N": kin, "K": M, "ms_med": med, "ms_best": best,
-                     "tflops": flops / med / 1e9, "frac_of_measured_peak": flops / med / 1e9 / PEAK_TF})
+        rows.append({"kernel": f"wgmma {name} sk={sk}", "M": nout, "N": kin, "K": M, "ms_med": med, "ms_best": best,
+                     "tflops": flops / med / 1e9, "frac_of_measured_peak": frac(flops / med / 1e9, PEAK_TF)})
         dwb = torch.empty(nout, kin, device="cuda", dtype=torch.bfloat16)
         med, best = timeit(lambda: torch.matmul(dy.t(), x, out=dwb))
         rows.append({"kernel": f"cublas  {name}", "M": nout, "N": kin, "K": M, "ms_med": med, "ms_best": best,
-                     "tflops": flops / med / 1e9, "frac_of_measured_peak": flops / med / 1e9 / PEAK_TF})
+                     "tflops": flops / med / 1e9, "frac_of_measured_peak": frac(flops / med / 1e9, PEAK_TF)})
 
     # memory-bound kernels
     x = torch.randn(M, C, device="cuda").bfloat16()
@@ -109,14 +114,14 @@ def main():
     med, best = timeit(lambda: F.layernorm_fwd(x, g, bta, y, mean, rstd))
     byts = 2 * M * C * 2
     rows.append({"kernel": "layernorm fwd", "ms_med": med, "ms_best": best, "gbs": byts / med / 1e6,
-                 "frac_of_measured_peak": byts / med / 1e6 / PEAK_BW})
+                 "frac_of_measured_peak": frac(byts / med / 1e6, PEAK_BW)})
     dx = torch.empty_like(x)
     dg = torch.zeros(C, device="cuda")
     dbt = torch.zeros(C, device="cuda")
     med, best = timeit(lambda: F.layernorm_bwd(y, x, g, mean, rstd, dx, dg, dbt, dres=x))
     byts = 4 * M * C * 2
     rows.append({"kernel": "layernorm bwd(+dres)", "ms_med": med, "ms_best": best, "gbs": byts / med / 1e6,
-                 "frac_of_measured_peak": byts / med / 1e6 / PEAK_BW})
+                 "frac_of_measured_peak": frac(byts / med / 1e6, PEAK_BW)})
     Vp = 50304
     logits = torch.randn(M, Vp, device="cuda").bfloat16()
     tgt = torch.randint(0, 50257, (M,), device="cuda")
@@ -124,7 +129,7 @@ def main():
     med, best = timeit(lambda: F.softmax_xent(logits, tgt, loss, 50257, 1.0 / M), iters=5)
     byts = 2 * M * Vp * 2
     rows.append({"kernel": "softmax_xent fwd+bwd", "ms_med": med, "ms_best": best, "gbs": byts / med / 1e6,
-                 "frac_of_measured_peak": byts / med / 1e6 / PEAK_BW})
+                 "frac_of_measured_peak": frac(byts / med / 1e6, PEAK_BW)})
     del logits
     n = 124_475_904 // 256 * 256
     p = torch.randn(n, device="cuda")
@@ -137,7 +142,7 @@ def main():
     med, best = timeit(lambda: F.adamw(p, gr, m1, v1, p16, mask, lr=1e-4, step=3, sumsq_buf=ss, max_norm=1.0))
     byts = n * (16 + 16 + 2)
     rows.append({"kernel": "adamw flat (fp32 p,g,m,v + bf16 copy + zero g)", "ms_med": med, "ms_best": best,
-                 "gbs": byts / med / 1e6, "frac_of_measured_peak": byts / med / 1e6 / PEAK_BW})
+                 "gbs": byts / med / 1e6, "frac_of_measured_peak": frac(byts / med / 1e6, PEAK_BW)})
     med, best = timeit(lambda: F.sumsq(gr, ss))
     rows.append({"kernel": "sumsq", "ms_med": med, "ms_best": best, "gbs": n * 4 / med / 1e6,
                  "frac_of_measured_peak": n * 4 / med / 1e6 / PEAK_BW})

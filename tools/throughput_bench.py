@@ -158,6 +158,7 @@ def main():
         path = "profiles/control_plane_throughput.json"
         d = json.load(open(path)) if os.path.exists(path) else {}
         d["three_daemons_http"] = out
+        os.makedirs("profiles", exist_ok=True)
         json.dump(d, open(path, "w"), indent=1)
         return
     jobs = int(sys.argv[1]) if len(sys.argv) > 1 else 100

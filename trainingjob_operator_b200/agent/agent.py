@@ -1,4 +1,4 @@
-"""Node agent: the kube-scheduler + kubelet analogue for one 8xB200 box.
+"""Node agent: the kube-scheduler + kubelet analogue for one 8xH100 box.
 
 The reference has no such component -- it relies on Kubernetes to place pods, start containers and
 report ``pod.status`` (SURVEY.md L0, Appendix A).  On a single box those roles collapse into this

@@ -1,7 +1,7 @@
 """All-in-one single-box control plane: API server + node agent + N (leader-elected) operators.
 
 There is no such thing in the reference (it needs an external Kubernetes, SURVEY.md L0); on one
-8xB200 machine this is the deployment unit: ``python -m trainingjob_operator_b200.cmd.local up``
+8xH100 machine this is the deployment unit: ``python -m trainingjob_operator_b200.cmd.local up``
 starts everything in one process (or use the three binaries ``cmd.apiserver``, ``cmd.agent``,
 ``cmd.main`` separately -- e.g. two operators for leader fail-over).  ``LocalCluster`` is also what
 tests, ``bench.py`` and ``__graft_entry__.smoke`` use as "the public API a user calls".

@@ -7,7 +7,7 @@ bidirectional attention (``y = LN(x + Attn(x))``, ``x' = LN(y + MLP(y))``), and 
 decoder tied to the word embeddings plus its own bias) with the loss taken over the masked positions only (15 % of the
 tokens; unmasked positions carry label -1).  GELU is the tanh form (``gelu_new``), which is what the GEMM epilogues fuse.
 
-Everything runs on the kernels of ``ops/csrc``: tcgen05 GEMMs with fused bias / GELU / residual epilogues (forward and
+Everything runs on the kernels of ``ops/csrc``: wgmma GEMMs with fused bias / GELU / residual epilogues (forward and
 input gradients; the residual epilogue of the dgrad GEMMs adds the skip connection's gradient), split-K weight-gradient
 GEMMs into the flat fp32 gradient buffer, LayerNorm forward / backward (the backward also yields the bias gradient of the
 linear layer in front of it), three-table embedding gather / scatter, softmax-cross-entropy with ignored labels, flat AdamW.
@@ -123,7 +123,7 @@ class BertEngine(GPT2Engine):
     Reuses the GEMM front-ends, attention, optimizer and bucket logic of ``GPT2Engine``; the wiring is BERT's."""
 
     def __init__(self, cfg: BertConfig, batch_size: int, seq_len: int, device="cuda", seed: int = 0,
-                 gemm_backend: str = "tcgen05"):
+                 gemm_backend: str = "wgmma"):
         from ..ops import functional as F
         import os
 
@@ -136,9 +136,9 @@ class BertEngine(GPT2Engine):
         self.backend = gemm_backend
         self.causal = False
         self.attn_impl = os.environ.get("AITJ_ATTN", "cudnn")
-        if self.attn_impl == "tcgen05" and (seq_len % 128 or cfg.n_embd // cfg.n_head != 64 or gemm_backend != "tcgen05"):
+        if self.attn_impl == "wgmma" and (seq_len % 128 or cfg.n_embd // cfg.n_head != 64 or gemm_backend != "wgmma"):
             self.attn_impl = "cudnn"
-        self.attn_bwd_impl = os.environ.get("AITJ_ATTN_BWD", "cudnn") if self.attn_impl == "tcgen05" else "cudnn"
+        self.attn_bwd_impl = os.environ.get("AITJ_ATTN_BWD", "cudnn") if self.attn_impl == "wgmma" else "cudnn"
         self._attn_delta = None
         self._dq_acc = None
         self._philox = torch.zeros((), dtype=torch.int64, device=device)
@@ -174,7 +174,7 @@ class BertEngine(GPT2Engine):
         self._dyn_host = torch.zeros(4, dtype=torch.float32).pin_memory() if self.dev.type == "cuda" else None
         self.pair = os.environ.get("AITJ_GEMM_PAIR", "1") != "0"
         self.gemm_cfg = {}
-        self.wgrad_stream = torch.cuda.Stream() if (self.dev.type == "cuda" and gemm_backend == "tcgen05" and
+        self.wgrad_stream = torch.cuda.Stream() if (self.dev.type == "cuda" and gemm_backend == "wgmma" and
                                                     os.environ.get("AITJ_WGRAD_STREAM", "0") != "0") else None
         self._wgrad_done = None
         self.segment_join = False

@@ -1,7 +1,7 @@
 """Flat parameter / gradient / optimizer-state storage for the hand-written training engines.
 
-Everything a worker trains lives in five contiguous device buffers laid out for 180 GB of HBM3e and
-one-sweep kernels: fp32 master weights ``p32``, their bf16 compute copy ``p16`` (what the tcgen05
+Everything a worker trains lives in five contiguous device buffers laid out for 80 GB of HBM3 and
+one-sweep kernels: fp32 master weights ``p32``, their bf16 compute copy ``p16`` (what the wgmma
 GEMMs read through TMA), fp32 gradients ``g32`` (wgrad GEMMs ``red.add`` into it, split-K and
 micro-batches accumulate for free), and AdamW moments ``m`` / ``v``.  Tensors are padded to 256
 elements so the per-256-element weight-decay mask of the AdamW kernel lines up, and the contiguous

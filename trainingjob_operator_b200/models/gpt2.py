@@ -1,9 +1,9 @@
-"""GPT-2 training engine written B200-first: explicit forward/backward over preallocated buffers.
+"""GPT-2 training engine written for H100: explicit forward/backward over preallocated buffers.
 
 This is one of the benchmark workloads BASELINE.json names ("GPT-2 small DDP"); the reference
 operator itself contains no model code (SURVEY.md §2.6).  There is no autograd tape and no tracing
-compiler on the hot path: every Linear is the hand-written tcgen05/TMA GEMM
-(``ops/csrc/gemm_tcgen05.cu``) with its bias / GELU / dGELU / residual epilogue fused, weight gradients
+compiler on the hot path: every Linear is the hand-written wgmma/TMA GEMM
+(``ops/csrc/gemm_wgmma.cu``) with its bias / GELU / dGELU / residual epilogue fused, weight gradients
 are split-K GEMMs that ``red.add`` straight into the flat fp32 gradient buffer, LayerNorm, embedding,
 softmax-cross-entropy and AdamW are single-sweep kernels (``ops/csrc/fused_ops.cu``), and the whole
 step is captured in one CUDA graph.  Only scaled-dot-product attention calls a library kernel
@@ -24,18 +24,12 @@ import torch.nn.functional as TF
 from .flat_params import FlatParams, ParamSpec
 
 
-# measured per-shape kernel choices (kind:NxK -> (block_n, split_k)) for the GPT-2 small step; everything else uses the CTA
-# pair wherever a 256x256 tile fits.  From tools/gemm_cfg_sweep.py (one change at a time in the captured step, same box,
-# profiles/r2_gemm_cfg_sweep.md): the 1-CTA 128x256 kernel wins where the epilogue is light and N is not a multiple of the
-# pair's wave (qkv / fc / lm_head forward, the proj and qkv input gradients), -0.03 .. -0.11 ms each.
-_DEFAULT_GEMM_CFG: Dict[str, Tuple[int, int]] = {
-    "fwd:2304x768": (256, 0), "fwd:3072x768": (256, 0), "fwd:50304x768": (256, 0),
-    "dgrad:768x768": (256, 0), "dgrad:768x2304": (256, 0),
-}
+# per-shape kernel choices (kind:NxK -> (block_n, split_k)) that override the default (the 2-CTA cluster wherever a
+# 256x256 cluster tile fits); tools/gemm_cfg_sweep.py measures candidates in the captured step.  None is set by default.
+_DEFAULT_GEMM_CFG: Dict[str, Tuple[int, int]] = {}
 
 _QKV_GATHER = os.environ.get("AITJ_QKV_GATHER", "1") != "0"
-_FUSE_COLSUM = os.environ.get("AITJ_FUSE_COLSUM", "1") != "0" and os.environ.get("AITJ_GEMM_EPI_WARPS", "16") != "8" \
-    and os.environ.get("AITJ_GEMM_GROUP_STORE", "0") == "0"
+_FUSE_COLSUM = os.environ.get("AITJ_FUSE_COLSUM", "1") != "0"
 
 
 @dataclass
@@ -107,14 +101,14 @@ class _LayerBufs:
         self.res2 = torch.empty(M, C, **bf)
         self.sdpa_ctx = None
         self.att_in = self.att
-        self.lse = None              # [B, H, T] fp32, only with the tcgen05 attention forward
+        self.lse = None              # [B, H, T] fp32, only with the wgmma attention forward
 
 
 class GPT2Engine:
     """Explicit fwd/bwd/optimizer for a fixed (B, T) micro-batch on one GPU."""
 
     def __init__(self, cfg: GPT2Config, batch_size: int, seq_len: int, device="cuda", seed: int = 0,
-                 gemm_backend: str = "tcgen05", causal: bool = True):
+                 gemm_backend: str = "wgmma", causal: bool = True):
         from ..ops import functional as F
 
         assert seq_len <= cfg.block_size and cfg.n_embd % 256 == 0
@@ -124,15 +118,14 @@ class GPT2Engine:
         self.M = batch_size * seq_len
         self.dev = torch.device(device)
         self.backend = gemm_backend
-        # attention forward: "cudnn" (PyTorch SDPA -> cuDNN flash kernel, the faster one today: 56 us per layer at
-        # B=16, T=1024) or "tcgen05" (our kernel, 71 us; AITJ_ATTN=tcgen05).  The backward is cuDNN's in both cases.
+        # attention forward: "cudnn" (PyTorch SDPA -> cuDNN flash kernel) or "wgmma" (our kernel, AITJ_ATTN=wgmma).
         self.attn_impl = os.environ.get("AITJ_ATTN", "cudnn")
-        if self.attn_impl == "tcgen05" and (seq_len % 128 or cfg.n_embd // cfg.n_head != 64 or gemm_backend != "tcgen05"):
+        if self.attn_impl == "wgmma" and (seq_len % 128 or cfg.n_embd // cfg.n_head != 64 or gemm_backend != "wgmma"):
             self.attn_impl = "cudnn"
-        # attention backward: "tcgen05" (ops/csrc/attention_bwd_tcgen05.cu: dq/dk/dv written straight into the packed d_qkv)
-        # needs our forward's log-sum-exp, so it implies the tcgen05 forward; "cudnn" = library kernel + gather
+        # attention backward: "wgmma" (ops/csrc/attention_bwd_wgmma.cu: dq/dk/dv written straight into the packed d_qkv)
+        # needs our forward's log-sum-exp, so it implies the wgmma forward; "cudnn" = library kernel + gather
         self.attn_bwd_impl = os.environ.get("AITJ_ATTN_BWD", "cudnn")
-        if self.attn_impl != "tcgen05":
+        if self.attn_impl != "wgmma":
             self.attn_bwd_impl = "cudnn"
         self._attn_delta = None
         self._dq_acc = None
@@ -170,17 +163,17 @@ class GPT2Engine:
         self._dyn_host = torch.zeros(4, dtype=torch.float32).pin_memory() if self.dev.type == "cuda" else None
         import os as _os
 
-        # CTA-pair (cta_group::2) GEMM: 256x256 tile per 2-CTA cluster (AITJ_GEMM_PAIR=0 falls back to 1-CTA)
+        # 2-CTA cluster GEMM: two 128x256 tiles sharing the B tile by TMA multicast (AITJ_GEMM_PAIR=0: single CTAs)
         self.pair = _os.environ.get("AITJ_GEMM_PAIR", "1") != "0"
         # per-GEMM kernel choice measured in the step (tools/gemm_cfg_sweep.py): "kind:NxK=block_n[/split_k]" entries,
-        # block_n 512 = CTA pair, 256 / 128 = 1-CTA tiles; AITJ_GEMM_CFG overrides / extends the table
+        # block_n 512 = 2-CTA cluster, 256 / 128 = 1-CTA tiles; AITJ_GEMM_CFG overrides / extends the table
         self.gemm_cfg: Dict[str, Tuple[int, int]] = dict(_DEFAULT_GEMM_CFG)
         for item in filter(None, _os.environ.get("AITJ_GEMM_CFG", "").split(",")):
             k, v = item.split("=")
             bn, _, sk = v.partition("/")
             self.gemm_cfg[k.strip()] = (int(bn), int(sk or 0))
         # weight-gradient GEMMs on a side stream (AITJ_WGRAD_STREAM=0: in line); see _wgrad
-        self.wgrad_stream = torch.cuda.Stream() if (self.dev.type == "cuda" and gemm_backend == "tcgen05" and
+        self.wgrad_stream = torch.cuda.Stream() if (self.dev.type == "cuda" and gemm_backend == "wgmma" and
                                                     _os.environ.get("AITJ_WGRAD_STREAM", "0") != "0") else None
         self._wgrad_done = None
         self.segment_join = False     # True: every backward segment joins the side stream (segments are separate graphs)
@@ -195,7 +188,7 @@ class GPT2Engine:
     # ------------------------------------------------------------------ GEMM front-ends
     def _linear(self, x, w, out, bias=None, residual=None, gelu=False, aux=None):
         F = self.F
-        if self.backend == "tcgen05":
+        if self.backend == "wgmma":
             F.gemm(x, w, out, bias=bias, residual=residual, gelu=gelu, save_pre=gelu, aux=aux,
                    block_n=self._bn(x.shape[0], w.shape[0], f"fwd:{w.shape[0]}x{w.shape[1]}"))
             return out
@@ -211,7 +204,7 @@ class GPT2Engine:
         return out
 
     def _bn(self, m: int, n: int, key: str = "") -> int:
-        """512 = CTA-pair kernel when the problem has at least one full 256x256 tile, else auto 1-CTA; a measured
+        """512 = 2-CTA cluster kernel when the problem has at least one full 256x256 cluster tile, else auto 1-CTA; a measured
         per-shape choice in ``gemm_cfg`` wins."""
         if key in self.gemm_cfg:
             return self.gemm_cfg[key][0]
@@ -221,7 +214,7 @@ class GPT2Engine:
         """out[M,K] = dy[M,N] @ w[N,K]  (* gelu'(aux)) (+ residual: the gradient arriving over a skip connection);
         colsum (fp32[K], optional) += column sums of out."""
         F = self.F
-        if self.backend == "tcgen05":
+        if self.backend == "wgmma":
             bn = self._bn(dy.shape[0], w.shape[1], f"dgrad:{w.shape[1]}x{w.shape[0]}")
             fused = colsum is not None and bn == 512 and _FUSE_COLSUM
             F.gemm(dy, w, out, b_mn=True, dgelu=dgelu_aux is not None, aux=dgelu_aux, residual=residual,
@@ -271,7 +264,7 @@ class GPT2Engine:
 
     def _wgrad_now(self, dy, x, dw):
         F = self.F
-        if self.backend == "tcgen05":
+        if self.backend == "wgmma":
             key = (dw.shape[0], dw.shape[1])
             if getattr(dw, "is_multicast", False):
                 # fused wgrad -> all-reduce: partial sums would each cross the switch, so no split-K; narrower tiles
@@ -296,8 +289,8 @@ class GPT2Engine:
     def _attention_fwd(self, lb: _LayerBufs):
         B, T, H = self.B, self.T, self.cfg.n_head
         D = self.cfg.n_embd // H
-        if self.attn_impl == "tcgen05":
-            # hand-written flash-attention forward (ops/csrc/attention_tcgen05.cu): reads the packed qkv in place,
+        if self.attn_impl == "wgmma":
+            # hand-written flash-attention forward (ops/csrc/attention_wgmma.cu): reads the packed qkv in place,
             # writes [B*T, H*D] and the log-sum-exp the backward needs
             if lb.lse is None:
                 lb.lse = torch.empty(B, H, T, device=self.dev, dtype=torch.float32)
@@ -322,7 +315,7 @@ class GPT2Engine:
         """d_qkv <- SDPA backward; d_bias (the qkv bias gradient) += colsum(d_qkv), fused into the gather."""
         B, T, H = self.B, self.T, self.cfg.n_head
         D = self.cfg.n_embd // H
-        if self.attn_bwd_impl == "tcgen05":
+        if self.attn_bwd_impl == "wgmma":
             if self._dq_acc is None:
                 self._attn_delta = torch.empty(B, H, T, device=self.dev, dtype=torch.float32)
                 self._dq_acc = torch.zeros(B * T, H * D, device=self.dev, dtype=torch.float32)
@@ -331,7 +324,7 @@ class GPT2Engine:
             self.F.colsum(d_qkv, d_bias)
             return
         do = d_att.view(B, T, H, D).transpose(1, 2)
-        if self.attn_impl == "tcgen05":
+        if self.attn_impl == "wgmma":
             # cuDNN's SDPA backward accepts our forward's output and log-sum-exp ([B,H,T,1], natural log)
             qkv5 = lb.qkv.view(B, T, 3, H, D)
             q, k, v = (qkv5[:, :, i].transpose(1, 2) for i in range(3))

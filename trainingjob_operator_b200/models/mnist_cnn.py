@@ -1,5 +1,5 @@
 """MNIST CNN (the PyTorch ``examples/mnist`` network) -- BASELINE.json config "torch DDP MNIST CNN
-AITrainingJob on 8xB200", and the stand-in for the reference's only example workload
+AITrainingJob on 8xH100", and the stand-in for the reference's only example workload
 (/root/reference/example/paddle-mnist.yaml:20-21 runs Paddle's recognize_digits).  Synthetic 1x28x28
 images, random-init weights; trained through ``parallel.flat_ddp`` with bf16 autocast on CUDA."""
 from __future__ import annotations

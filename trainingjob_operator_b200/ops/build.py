@@ -1,9 +1,9 @@
-"""In-tree build of the sm_100a kernel library and the native control-plane core.
+"""In-tree build of the sm_90a (H100) kernel library and the native control-plane core.
 
-Two artefacts, both left next to their sources so they travel with a `gpurun` snapshot:
+Two artefacts, both left next to their sources inside the package, so the package runs from the source tree:
 
 * ``ops/libaitj_kernels.so``  -- every ``ops/csrc/*.cu`` compiled by ``nvcc`` for
-  ``compute_100a/sm_100a`` with ``-lineinfo`` (plain C ABI, loaded through ``ctypes``; no
+  ``compute_90a/sm_90a`` with ``-lineinfo`` (plain C ABI, loaded through ``ctypes``; no
   dependency on torch's C++ ABI, so a rebuild takes seconds).
 * ``core/_aitj_core*.so``     -- the C++17 control-plane runtime (work-queue, object store,
   process supervisor) as a pybind11 module.
@@ -28,7 +28,7 @@ CORE_DIR = PKG / "core"
 KERNEL_LIB = OPS_DIR / "libaitj_kernels.so"
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC",
     "-Xptxas", "-v",
@@ -50,7 +50,7 @@ def _digest(paths) -> str:
 
 
 def build_kernels(force: bool = False, verbose: bool = False) -> Path:
-    """Compile ops/csrc/*.cu into ops/libaitj_kernels.so (sm_100a)."""
+    """Compile ops/csrc/*.cu into ops/libaitj_kernels.so (sm_90a)."""
     sources = sorted(CSRC.glob("*.cu"))
     headers = sorted(CSRC.glob("*.cuh"))
     stamp = OPS_DIR / ".kernels.sha256"
@@ -59,7 +59,7 @@ def build_kernels(force: bool = False, verbose: bool = False) -> Path:
         return KERNEL_LIB
     nvcc = _nvcc()
     if nvcc is None:
-        raise RuntimeError("nvcc not found; cannot build sm_100a kernels")
+        raise RuntimeError("nvcc not found; cannot build sm_90a kernels")
     objs = []
     build_dir = OPS_DIR / "build"
     build_dir.mkdir(exist_ok=True)

@@ -1,4 +1,4 @@
-// Memory-bound fused kernels of the worker training step (sm_100a): LayerNorm fwd/bwd,
+// Memory-bound fused kernels of the worker training step (sm_90a): LayerNorm fwd/bwd,
 // embedding fwd/bwd, softmax-cross-entropy fwd+bwd in one pass, bias-grad column reduce,
 // flat-buffer AdamW (fp32 master + bf16 compute copy + grad zeroing in one sweep),
 // grad-norm, casts.  All 16-byte vectorised; one HBM read + one write per tensor.
@@ -622,6 +622,17 @@ __global__ void __launch_bounds__(256) gelu_bwd_kernel(const __nv_bfloat16* __re
   }
 }
 
+// SM count of the current device: grids are capped at a few CTAs per SM and loop over the rest
+static int sms() {
+  static int n = 0;
+  if (!n) {
+    int dev = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
+  }
+  return n;
+}
+
 static int grid_for(size_t work_items, int threads, int max_blocks) {
   size_t b = (work_items + threads - 1) / threads;
   if (b > static_cast<size_t>(max_blocks)) b = max_blocks;
@@ -641,7 +652,7 @@ using namespace aitj;
 int aitj_layernorm_fwd(const void* x, const void* gamma, const void* beta, void* y, void* mean, void* rstd, int M,
                        int C, float eps, void* stream) {
   if (C % 256 || C > 2048) return -1;
-  const int blocks = min((M + 7) / 8, 148 * 2);
+  const int blocks = min((M + 7) / 8, sms() * 2);
 #define LN_F(V) layernorm_fwd_kernel<V><<<blocks, 256, 0, S(stream)>>>(CBF(x), CBF(gamma), CBF(beta), BF(y), \
     reinterpret_cast<float*>(mean), reinterpret_cast<float*>(rstd), M, eps)
   switch (C / 256) {
@@ -656,7 +667,7 @@ int aitj_layernorm_bwd(const void* dy, const void* x, const void* gamma, const v
                        const void* dres, void* dx, void* dgamma, void* dbeta, void* dxsum, int M, int C, int mc,
                        void* stream) {
   if (C % 256 || C > 1024) return -1;
-  const int blocks = min((M + kLnBwdWarps - 1) / kLnBwdWarps, 148);
+  const int blocks = min((M + kLnBwdWarps - 1) / kLnBwdWarps, sms());
 #define LN_B(V) layernorm_bwd_kernel<V><<<blocks, kLnBwdWarps * 32, 0, S(stream)>>>(CBF(dy), CBF(x), CBF(gamma), \
     reinterpret_cast<const float*>(mean), reinterpret_cast<const float*>(rstd), CBF(dres), BF(dx), \
     reinterpret_cast<float*>(dgamma), reinterpret_cast<float*>(dbeta), reinterpret_cast<float*>(dxsum), M, mc)
@@ -672,7 +683,7 @@ int aitj_embedding_fwd(const void* tok, const void* wte, const void* wpe, void* 
                        void* stream) {
   if (C % 8) return -1;
   const size_t total = static_cast<size_t>(M) * (C / 8);
-  embedding_fwd_kernel<<<grid_for(total, 256, 148 * 16), 256, 0, S(stream)>>>(
+  embedding_fwd_kernel<<<grid_for(total, 256, sms() * 16), 256, 0, S(stream)>>>(
       reinterpret_cast<const int64_t*>(tok), CBF(wte), CBF(wpe), BF(out), M, T, C);
   return LAUNCH_OK();
 }
@@ -681,7 +692,7 @@ int aitj_embedding_bwd(const void* tok, const void* dx, void* dwte, void* dwpe, 
                        void* stream) {
   if (C % 4) return -1;
   const size_t total = static_cast<size_t>(M) * (C / 4);
-  embedding_bwd_kernel<<<grid_for(total, 256, 148 * 16), 256, 0, S(stream)>>>(
+  embedding_bwd_kernel<<<grid_for(total, 256, sms() * 16), 256, 0, S(stream)>>>(
       reinterpret_cast<const int64_t*>(tok), CBF(dx), reinterpret_cast<float*>(dwte), reinterpret_cast<float*>(dwpe),
       M, T, C, mc);
   return LAUNCH_OK();
@@ -692,7 +703,7 @@ int aitj_embedding3_fwd(const void* tok, const void* typ, const void* wte, const
                         int M, int T, int C, void* stream) {
   if (C % 8) return -1;
   const size_t total = static_cast<size_t>(M) * (C / 8);
-  embedding_fwd_kernel<<<grid_for(total, 256, 148 * 16), 256, 0, S(stream)>>>(
+  embedding_fwd_kernel<<<grid_for(total, 256, sms() * 16), 256, 0, S(stream)>>>(
       reinterpret_cast<const int64_t*>(tok), CBF(wte), CBF(wpe), BF(out), M, T, C,
       reinterpret_cast<const int64_t*>(typ), CBF(wtt));
   return LAUNCH_OK();
@@ -702,7 +713,7 @@ int aitj_embedding3_bwd(const void* tok, const void* typ, const void* dx, void* 
                         int C, int mc, void* stream) {
   if (C % 4) return -1;
   const size_t total = static_cast<size_t>(M) * (C / 4);
-  embedding_bwd_kernel<<<grid_for(total, 256, 148 * 16), 256, 0, S(stream)>>>(
+  embedding_bwd_kernel<<<grid_for(total, 256, sms() * 16), 256, 0, S(stream)>>>(
       reinterpret_cast<const int64_t*>(tok), CBF(dx), reinterpret_cast<float*>(dwte), reinterpret_cast<float*>(dwpe),
       M, T, C, mc, reinterpret_cast<const int64_t*>(typ), reinterpret_cast<float*>(dwtt));
   return LAUNCH_OK();
@@ -711,10 +722,8 @@ int aitj_embedding3_bwd(const void* tok, const void* typ, const void* dx, void* 
 int aitj_softmax_xent(void* logits, const void* target, void* loss, int M, int V, int Vp, float gscale,
                       void* stream) {
   if (Vp % 8 || V > Vp) return -1;
-  // Three alternatives were measured slower at 16384 x 50304 and removed (profiles/README.md): the row held in registers
-  // by one 1024-thread CTA (1.99 ms: nothing overlaps a row's load), a 2-CTA cluster holding half a row each (0.89 ms:
-  // the DSMEM exchanges cost more than the extra residency buys) and a persistent 1024-thread CTA with bulk-async row
-  // prefetch / store (1.02 ms).  This kernel -- row staged in shared memory, two CTAs per SM -- takes 0.84 ms.
+  // The row is staged in shared memory (100 KB at Vp = 50304, so two CTAs fit an SM's 228 KB): one HBM read and one
+  // write per logit, and the second CTA's loads overlap the first one's exponentials.
   const int smem = Vp * 2;
   if (smem > 200 * 1024) return -2;
   static int configured = 0;
@@ -732,7 +741,7 @@ int aitj_colsum(const void* dy, void* db, int M, int N, int mc, void* stream) {
   if (N % 8) return -1;
   const int col_blocks = (N + 255) / 256;
   int rows_per_block = 512;
-  while (rows_per_block > 32 && col_blocks * ((M + rows_per_block - 1) / rows_per_block) < 148 * 4) rows_per_block /= 2;
+  while (rows_per_block > 32 && col_blocks * ((M + rows_per_block - 1) / rows_per_block) < sms() * 4) rows_per_block /= 2;
   dim3 grid(col_blocks, (M + rows_per_block - 1) / rows_per_block);
   colsum_kernel<<<grid, 256, 0, S(stream)>>>(CBF(dy), reinterpret_cast<float*>(db), M, N, rows_per_block, mc);
   return LAUNCH_OK();
@@ -748,7 +757,7 @@ int aitj_qkv_gather_colsum(const void* dq, const void* dk, const void* dv, const
   const int M = B * T, C = H * D, N = 3 * C;
   const int col_blocks = (N + 255) / 256;
   int rows_per_block = 512;
-  while (rows_per_block > 32 && col_blocks * ((M + rows_per_block - 1) / rows_per_block) < 148 * 4) rows_per_block /= 2;
+  while (rows_per_block > 32 && col_blocks * ((M + rows_per_block - 1) / rows_per_block) < sms() * 4) rows_per_block /= 2;
   dim3 grid(col_blocks, (M + rows_per_block - 1) / rows_per_block);
   qkv_gather_colsum_kernel<<<grid, 256, 0, S(stream)>>>(src, BF(out), reinterpret_cast<float*>(db), M, T, C, D,
                                                          rows_per_block, mc);
@@ -757,7 +766,7 @@ int aitj_qkv_gather_colsum(const void* dq, const void* dk, const void* dv, const
 
 int aitj_sumsq(const void* g, long long n, void* out, void* stream) {
   if (n % 4) return -1;
-  sumsq_kernel<<<grid_for(static_cast<size_t>(n) / 4, 512, 148 * 4), 512, 0, S(stream)>>>(
+  sumsq_kernel<<<grid_for(static_cast<size_t>(n) / 4, 512, sms() * 4), 512, 0, S(stream)>>>(
       reinterpret_cast<const float*>(g), static_cast<size_t>(n), reinterpret_cast<float*>(out));
   return LAUNCH_OK();
 }
@@ -778,7 +787,7 @@ int aitj_fused_set_peers(const void* base, const long long* delta, const long lo
 
 int aitj_peer_push(void* dst_local, void* src, long long n, void* stream) {
   if (n % 4) return -1;
-  peer_push_kernel<<<grid_for(static_cast<size_t>(n) / 4, 256, 148 * 2), 256, 0, S(stream)>>>(
+  peer_push_kernel<<<grid_for(static_cast<size_t>(n) / 4, 256, sms() * 2), 256, 0, S(stream)>>>(
       reinterpret_cast<float*>(dst_local), reinterpret_cast<float*>(src), static_cast<size_t>(n));
   return LAUNCH_OK();
 }
@@ -800,7 +809,7 @@ int aitj_adamw(void* p, void* g, void* m, void* v, void* p16, const void* wd_mas
   a.bc1 = 1.0f - powf(beta1, static_cast<float>(step));
   a.bc2 = 1.0f - powf(beta2, static_cast<float>(step));
   a.max_norm = max_norm; a.grad_div = grad_div; a.zero_grad = zero_grad;
-  adamw_kernel<<<grid_for(static_cast<size_t>(n) / 4, 256, 148 * 8), 256, 0, S(stream)>>>(
+  adamw_kernel<<<grid_for(static_cast<size_t>(n) / 4, 256, sms() * 8), 256, 0, S(stream)>>>(
       reinterpret_cast<float*>(p), reinterpret_cast<float*>(g), reinterpret_cast<float*>(m),
       reinterpret_cast<float*>(v), BF(p16), reinterpret_cast<const uint8_t*>(wd_mask),
       reinterpret_cast<const float*>(sumsq), reinterpret_cast<const float*>(dyn), static_cast<size_t>(n), a);
@@ -809,27 +818,27 @@ int aitj_adamw(void* p, void* g, void* m, void* v, void* p16, const void* wd_mas
 
 int aitj_mc_push(void* dst_mc, void* src, long long n, void* stream) {
   if (n % 4) return -1;
-  mc_push_kernel<<<grid_for(static_cast<size_t>(n) / 4, 256, 148 * 2), 256, 0, S(stream)>>>(
+  mc_push_kernel<<<grid_for(static_cast<size_t>(n) / 4, 256, sms() * 2), 256, 0, S(stream)>>>(
       reinterpret_cast<float*>(dst_mc), reinterpret_cast<float*>(src), static_cast<size_t>(n));
   return LAUNCH_OK();
 }
 
 int aitj_cast_f32_bf16(const void* in, void* out, long long n, void* stream) {
   if (n % 4) return -1;
-  cast_f32_bf16_kernel<<<grid_for(static_cast<size_t>(n) / 4, 256, 148 * 8), 256, 0, S(stream)>>>(
+  cast_f32_bf16_kernel<<<grid_for(static_cast<size_t>(n) / 4, 256, sms() * 8), 256, 0, S(stream)>>>(
       reinterpret_cast<const float*>(in), BF(out), static_cast<size_t>(n));
   return LAUNCH_OK();
 }
 
 int aitj_gelu_fwd(const void* x, void* y, long long n, void* stream) {
   if (n % 8) return -1;
-  gelu_fwd_kernel<<<grid_for(static_cast<size_t>(n) / 8, 256, 148 * 8), 256, 0, S(stream)>>>(CBF(x), BF(y),
+  gelu_fwd_kernel<<<grid_for(static_cast<size_t>(n) / 8, 256, sms() * 8), 256, 0, S(stream)>>>(CBF(x), BF(y),
                                                                                              static_cast<size_t>(n));
   return LAUNCH_OK();
 }
 int aitj_gelu_bwd(const void* x, const void* dy, void* dx, long long n, void* stream) {
   if (n % 8) return -1;
-  gelu_bwd_kernel<<<grid_for(static_cast<size_t>(n) / 8, 256, 148 * 8), 256, 0, S(stream)>>>(
+  gelu_bwd_kernel<<<grid_for(static_cast<size_t>(n) / 8, 256, sms() * 8), 256, 0, S(stream)>>>(
       CBF(x), CBF(dy), BF(dx), static_cast<size_t>(n));
   return LAUNCH_OK();
 }

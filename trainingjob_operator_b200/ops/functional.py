@@ -1,4 +1,4 @@
-"""Python entry points of the hand-written sm_100a kernels (ctypes -> libaitj_kernels.so).
+"""Python entry points of the hand-written sm_90a kernels (ctypes -> libaitj_kernels.so).
 
 Every function launches on ``torch.cuda.current_stream()`` and works on preallocated
 tensors, so a whole training step can be captured in one CUDA graph.  There is deliberately
@@ -89,15 +89,16 @@ def _ptr(t):
 
 
 def gemm(a, b, out, *, a_mn=False, b_mn=False, bias=None, residual=None, aux=None, gelu=False, dgelu=False,
-         save_pre=False, accumulate=False, split_k=1, block_n=0, max_ctas=0, colsum=None,
-         _debug_skip_epilogue=False):
-    """out[M,N] (+)= opA[M,K] @ opB[N,K]^T on tcgen05 tensor cores (bf16 in, fp32 accumulate).
+         save_pre=False, accumulate=False, split_k=1, block_n=0, max_ctas=0, colsum=None):
+    """out[M,N] (+)= opA[M,K] @ opB[N,K]^T on wgmma tensor cores (bf16 in, fp32 accumulate).
 
     a_mn=False: ``a`` is [M,K]; a_mn=True: ``a`` is [K,M] (its transpose is used).
     b_mn=False: ``b`` is [N,K]; b_mn=True: ``b`` is [K,N].
     ``out`` bf16 -> plain store; fp32 -> store, or red.add when ``accumulate`` (needed for split_k>1).
     Epilogue: +bias[N] -> (aux<-pre) -> gelu -> *gelu'(aux) -> +residual[M,N].
-    ``colsum`` (fp32[N], CTA-pair kernel with bf16 output only): += column sums of the stored output.
+    ``block_n``: 128 / 256 = tile width, 0 = auto, 512 / 1024 = 128x256 tiles in clusters of 2 / 4 CTAs that share the
+    B tile by TMA multicast.
+    ``colsum`` (fp32[N], bf16 output only): += column sums of the stored output.
     """
     assert a.dtype == torch.bfloat16 and b.dtype == torch.bfloat16
     assert a.dim() == 2 and b.dim() == 2 and a.stride(1) == 1 and b.stride(1) == 1 and out.stride(1) == 1
@@ -136,10 +137,8 @@ def gemm(a, b, out, *, a_mn=False, b_mn=False, bias=None, residual=None, aux=Non
     else:
         assert out.dtype == torch.bfloat16 and not accumulate
     if colsum is not None:
-        assert colsum.dtype == torch.float32 and colsum.numel() == N and block_n == 512
+        assert colsum.dtype == torch.float32 and colsum.numel() == N and out.dtype == torch.bfloat16
         lib.load().aitj_gemm_set_colsum(colsum.data_ptr())
-    if _debug_skip_epilogue:
-        flags |= {True: 256, "notma": 1024, "ldonly": 2048}[_debug_skip_epilogue]
     lib.call("aitj_gemm_bf16", a.data_ptr(), b.data_ptr(), out.data_ptr(), M, N, K, a.stride(0), b.stride(0),
              out.stride(0), int(a_mn), int(b_mn), _ptr(bias), _ptr(residual), _ptr(aux), flags, int(split_k),
              int(block_n), int(max_ctas), _stream())
@@ -226,7 +225,7 @@ def colsum(dy, db):
 
 
 def attention_fwd(qkv, out, lse, B, T, H, causal=True, scale=0.0):
-    """Flash attention forward on tcgen05 (head dim 64): qkv bf16 [B*T, 3*H*64] packed q|k|v -> out bf16 [B*T, H*64],
+    """Flash attention forward on wgmma (head dim 64): qkv bf16 [B*T, 3*H*64] packed q|k|v -> out bf16 [B*T, H*64],
     lse fp32 [B, H, T] (natural-log sum-exp of the scaled scores).  T % 128 == 0."""
     assert qkv.dtype == torch.bfloat16 and out.dtype == torch.bfloat16 and lse.dtype == torch.float32
     assert qkv.is_contiguous() and out.is_contiguous() and lse.is_contiguous()
@@ -237,7 +236,7 @@ def attention_fwd(qkv, out, lse, B, T, H, causal=True, scale=0.0):
 
 
 def attention_bwd(qkv, out, d_out, lse, delta, dq_acc, d_qkv, B, T, H, causal=True, scale=0.0):
-    """Flash attention backward on tcgen05 (head dim 64).  qkv / d_qkv bf16 [B*T, 3*H*64] (d_qkv receives dq | dk | dv in
+    """Flash attention backward on wgmma (head dim 64).  qkv / d_qkv bf16 [B*T, 3*H*64] (d_qkv receives dq | dk | dv in
     place), out / d_out bf16 [B*T, H*64], lse fp32 [B,H,T] from ``attention_fwd``; delta fp32 [B,H,T] and dq_acc fp32
     [B*T, H*64] are scratch -- dq_acc must be zero on entry and is zero again on exit."""
     assert qkv.dtype == torch.bfloat16 and d_qkv.dtype == torch.bfloat16 and dq_acc.dtype == torch.float32

@@ -1,4 +1,4 @@
-"""ctypes loader for ``libaitj_kernels.so`` (the hand-written sm_100a kernels).
+"""ctypes loader for ``libaitj_kernels.so`` (the hand-written sm_90a kernels).
 
 The library is a plain C ABI: every entry point takes raw device pointers and a CUDA stream
 handle and returns 0 or a negative error code.  ``check`` turns non-zero codes into
@@ -61,10 +61,8 @@ _F = ctypes.c_float
 _SIGS = {
     "aitj_gemm_bf16": [_P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _P, _P, _P, _I, _I, _I, _I, _P],
     "aitj_num_sms": [],
-    "aitj_attn_set_trace": [_P],
     "aitj_attn_fwd": [_P, _P, _P, _I, _I, _I, _I, _F, _P],
     "aitj_attn_bwd": [_P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _F, _P],
-    "aitj_gemm_set_trace": [_P],
     "aitj_gemm_set_colsum": [_P],
     "aitj_layernorm_fwd": [_P, _P, _P, _P, _P, _P, _I, _I, _F, _P],
     "aitj_layernorm_bwd": [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _P],

@@ -131,6 +131,25 @@ def case_gemm_epilogue():
     sk = F.auto_split_k(Nout, Kin, Mtok)
     F.gemm(dyv, x, dw, a_mn=True, b_mn=True, accumulate=True, split_k=sk)
     ok &= _check(f"wgrad split_k={sk}", dw, dyv.float().t() @ x.float(), 1e-2)
+    # owner-sharded weight gradient (EPI_PEER) with a second rank emulated on this GPU: the peer table maps the upper
+    # half of the flat buffer to another local allocation standing in for rank 1's copy.  Rows this rank owns are summed
+    # in place; the others arrive in the owner's copy, and the local copy of them is zero again afterwards.
+    import ctypes
+
+    ref = dyv.float().t() @ x.float()
+    half = Nout // 2
+    for sk_peer in (1, 4):
+        local = torch.zeros(Nout * Kin, device="cuda")
+        owner1 = torch.zeros(Nout * Kin, device="cuda")
+        delta = (ctypes.c_longlong * 8)(0, owner1.data_ptr() - local.data_ptr(), *([0] * 6))
+        bound = (ctypes.c_longlong * 9)(0, half * Kin, *([Nout * Kin] * 7))
+        assert F.lib.load().aitj_gemm_set_peers(ctypes.c_void_p(local.data_ptr()), delta, bound, 2) == 0
+        F.gemm(dyv, x, F.PeerView(local.view(Nout, Kin)), a_mn=True, b_mn=True, accumulate=True, split_k=sk_peer)
+        torch.cuda.synchronize()
+        lo, hi = local.view(Nout, Kin), owner1.view(Nout, Kin)
+        ok &= _check(f"peer wgrad split_k={sk_peer}: owned rows in place", lo[:half], ref[:half], 1e-2)
+        ok &= _check(f"peer wgrad split_k={sk_peer}: other rows at the owner", hi[half:], ref[half:], 1e-2)
+        ok &= bool((lo[half:] == 0).all()) and bool((hi[:half] == 0).all())
     torch.cuda.synchronize()
     return ok
 
@@ -167,7 +186,7 @@ def case_gemm_quad():
 
 
 def case_gemm_2cta():
-    """CTA-pair kernel (tcgen05.mma.cta_group::2, 256x256 tile per 2-CTA cluster): all layouts + epilogues."""
+    """CTA-pair kernel (wgmma, 256x256 tile per 2-CTA cluster): all layouts + epilogues."""
     ok = True
     for (M, N, K, a_mn, b_mn) in [(256, 256, 64, False, False), (256, 256, 256, False, False),
                                   (512, 768, 768, False, False), (1000, 776, 200, False, False),
@@ -327,7 +346,7 @@ def case_fused_ops():
 
 
 def case_gpt2_engine():
-    """Hand-written engine (tcgen05 GEMMs + fused kernels) vs the plain fp32 PyTorch model: loss and grads."""
+    """Hand-written engine (wgmma GEMMs + fused kernels) vs the plain fp32 PyTorch model: loss and grads."""
     from ..models.gpt2 import GPT2Config, GPT2Engine, GPT2Reference
 
     ok = True
@@ -335,15 +354,15 @@ def case_gpt2_engine():
     B, T = 4, 128
     import os
 
-    for backend, attn, attn_bwd in (("tcgen05", "cudnn", "cudnn"), ("cublas", "cudnn", "cudnn"),
-                                    ("tcgen05", "tcgen05", "cudnn"), ("tcgen05", "tcgen05", "tcgen05")):
+    for backend, attn, attn_bwd in (("wgmma", "cudnn", "cudnn"), ("cublas", "cudnn", "cudnn"),
+                                    ("wgmma", "wgmma", "cudnn"), ("wgmma", "wgmma", "wgmma")):
         os.environ["AITJ_ATTN"] = attn
         os.environ["AITJ_ATTN_BWD"] = attn_bwd
         eng = GPT2Engine(cfg, B, T, "cuda", seed=3, gemm_backend=backend)
         os.environ.pop("AITJ_ATTN", None)
         os.environ.pop("AITJ_ATTN_BWD", None)
         assert eng.attn_impl == attn and eng.attn_bwd_impl == attn_bwd
-        backend = backend if attn == "cudnn" else backend + "+attn" + ("+attn_bwd" if attn_bwd == "tcgen05" else "")
+        backend = backend if attn == "cudnn" else backend + "+attn" + ("+attn_bwd" if attn_bwd == "wgmma" else "")
         ref = GPT2Reference(cfg, eng.params).cuda()
         g = torch.Generator().manual_seed(5)
         tok = torch.randint(0, cfg.vocab_size, (B, T), generator=g).cuda()
@@ -375,7 +394,7 @@ def case_gpt2_engine():
 
 
 def case_attention_bwd():
-    """tcgen05 flash-attention backward vs. autograd through an fp32 PyTorch attention on the same bf16 inputs (causal
+    """wgmma flash-attention backward vs. autograd through an fp32 PyTorch attention on the same bf16 inputs (causal
     and full), plus its device time next to the cuDNN SDPA backward PyTorch dispatches to."""
     ok = True
     for (B, T, H, causal) in [(1, 128, 1, True), (2, 256, 3, True), (2, 384, 2, False), (1, 1024, 4, True)]:
@@ -433,7 +452,7 @@ def case_attention_bwd():
     t_lib = timeit(lambda: torch.ops.aten._scaled_dot_product_cudnn_attention_backward(
         do4, q, k, v, o4, lse.view(B, H, T, 1), philox, philox, None, None, None, T, T, 0.0, True))
     flops = 10.0 * B * H * T * T * 64 / 2
-    print(f"  attention bwd B16 T1024 H12 causal: tcgen05 (delta + main + dq finish) {t_ours:.1f} us "
+    print(f"  attention bwd B16 T1024 H12 causal: wgmma (delta + main + dq finish) {t_ours:.1f} us "
           f"({flops / t_ours / 1e6:.0f} TFLOP/s)  cuDNN SDPA backward (no gather) {t_lib:.1f} us "
           f"({flops / t_lib / 1e6:.0f} TFLOP/s)")
     return ok
@@ -528,7 +547,7 @@ def case_bert_engine():
 
 # ----------------------------------------------------------------------------- attention
 def case_attention():
-    """tcgen05 flash-attention forward vs. an fp32 PyTorch reference (causal and full), plus its device time next to
+    """wgmma flash-attention forward vs. an fp32 PyTorch reference (causal and full), plus its device time next to
     the cuDNN SDPA kernel PyTorch dispatches to."""
     ok = True
     for (B, T, H, causal) in [(2, 256, 3, True), (1, 128, 2, True), (2, 384, 2, False), (2, 1024, 12, True),
@@ -576,7 +595,7 @@ def case_attention():
     q, k, v = (qkv.view(B, T, 3, H, 64)[:, :, i].transpose(1, 2) for i in range(3))
     t_lib = timeit(lambda: torch.nn.functional.scaled_dot_product_attention(q, k, v, is_causal=True))
     flops = 4.0 * B * H * T * T * 64 / 2
-    print(f"  attention fwd B16 T1024 H12 causal: tcgen05 {t_ours:.1f} us ({flops / t_ours / 1e6:.0f} TFLOP/s)  "
+    print(f"  attention fwd B16 T1024 H12 causal: wgmma {t_ours:.1f} us ({flops / t_ours / 1e6:.0f} TFLOP/s)  "
           f"cuDNN SDPA {t_lib:.1f} us ({flops / t_lib / 1e6:.0f} TFLOP/s)")
     return ok
 

@@ -3,7 +3,7 @@
 The DDP hot op is "weight-gradient GEMM followed by a gradient all-reduce".  Instead of calling a
 collective after the GEMM, the gradient buffer is allocated as CUDA symmetric memory with an NVLS
 multicast alias (``torch.distributed._symmetric_memory`` provides the allocation/rendezvous plumbing), and
-every gradient-producing kernel of the backward pass -- the tcgen05 wgrad GEMM epilogue, LayerNorm-backward,
+every gradient-producing kernel of the backward pass -- the wgmma wgrad GEMM epilogue, LayerNorm-backward,
 the bias column-reduce, the embedding scatter -- issues ``multimem.red.add`` on that alias: the NVSwitch
 applies each contribution to all peers' buffers while the math of the next tile proceeds.  When backward
 ends, every rank already holds the summed gradient; two device-side barriers per step replace all
@@ -90,7 +90,7 @@ class ShardedGradState:
     ``_symmetric_memory`` does the allocation / handle exchange), rank r owns the flat range ``bounds[r]:bounds[r+1]``,
     and
 
-    * every gradient producer -- the tcgen05 wgrad GEMM epilogue (``EPI_PEER``, split-K partials included), the
+    * every gradient producer -- the wgmma wgrad GEMM epilogue (``EPI_PEER``, split-K partials included), the
       embedding scatter, the pushed 1-D gradients -- ``red.add``s into the OWNER's copy over the peer mapping
       ((N-1)/N of the gradient bytes cross NVLink once; the multicast path delivered N x that);
     * the owner clips (partial square sums are exchanged with one multicast store each) and runs AdamW on its 1/N of

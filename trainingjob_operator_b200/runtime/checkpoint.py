@@ -7,7 +7,7 @@ image.  The bundled workers need one for ``restartScope: All`` / ``Replica`` res
 the step loop:
 
 1. *snapshot* on the training stream: one device-to-device copy per state tensor into buffers allocated once (GPT-2
-   small: 1.5 GB, ~0.4 ms of HBM traffic; 180 GB of HBM makes the second copy a non-issue).  It is ordered after the
+   small: 1.5 GB, ~1 ms of HBM traffic; with 80 GB of HBM the second copy is a small share).  It is ordered after the
    optimizer step that produced the state and before the next one by stream order, CUDA-graph replays included.
 2. *drain* on a side stream: device-to-host copies of the snapshot into pinned buffers, overlapping the following steps.
 3. *write* on a host thread: waits for the drain event, ``torch.save`` to ``<path>.tmp``, ``fsync``, atomic rename -- a

@@ -282,7 +282,7 @@ class TorchAdapter:
 def build_adapter(args, device: torch.device):
     if args.model in ("gpt2", "gpt2-tiny", "bert", "bert-tiny"):
         if device.type != "cuda":
-            raise RuntimeError(f"model {args.model} needs a CUDA device (hand-written sm_100a kernels)")
+            raise RuntimeError(f"model {args.model} needs a CUDA device (hand-written sm_90a kernels)")
         return EngineAdapter(args.model, args.batch, args.seq, args)
     return TorchAdapter(args.model, args.batch, args, device)
 
@@ -349,6 +349,24 @@ def guarded(breaker, generation: int, fn):
 
 
 # ------------------------------------------------------------------------------------ main loop
+def dump_outputs(out_dir: str, adapter, losses) -> None:
+    """What the timed steps computed, so that two builds can be compared output for output on the same seeded inputs:
+    ``losses.npy`` (float64, the loss of every timed step, the last one being the final step's) and ``weights_sample.npy``
+    (float32, 4 Mi elements of the fp32 master weights after the last step -- the state the step updates -- at indices
+    drawn from a fixed seed; all of them when the model is smaller).  With several ranks the caller first gathers the
+    whole state on every rank (``adapter.prepare_state()``), so the sample covers every rank's optimizer shard."""
+    import numpy as np
+
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "losses.npy"), np.asarray(losses, dtype=np.float64))
+    w = adapter.state_tensors()[0].detach().reshape(-1)
+    n = w.numel()
+    if n > (1 << 22):
+        idx = torch.randint(0, n, (1 << 22,), generator=torch.Generator().manual_seed(0)).sort().values
+        w = w[idx.to(w.device)]
+    np.save(os.path.join(out_dir, "weights_sample.npy"), w.float().cpu().numpy())
+
+
 def run(args) -> Dict[str, Any]:
     t_proc = time.time()
     rank = env_int("RANK", env_int("TRAININGJOB_REPLICA_INDEX", 0))
@@ -364,9 +382,8 @@ def run(args) -> Dict[str, Any]:
         # (TearDown / SkipCleanUp); a faultTolerant job handles the loss of a peer itself (StallBreaker + recovery below)
         os.environ.setdefault("TORCH_NCCL_ASYNC_ERROR_HANDLING", "0")
         # A communicator that must be abortable with a peer already dead should not hold NVSwitch multicast (NVLS)
-        # objects: their teardown involves every member.  Precaution, not a measured fix -- in-place recovery is verified
-        # on 2 GPUs (where NCCL does not use NVLS); the 4-GPU attempts of round 2 ended without a diagnosis
-        # (profiles/r2_fault_recovery_gpu.md).  Costs the faultTolerant job's all-reduce the in-switch reduction.
+        # objects: their teardown involves every member.  Precaution, not a measured fix.  Costs the faultTolerant job's
+        # all-reduce the in-switch reduction.
         os.environ.setdefault("NCCL_NVLS_ENABLE", "0")
     trace = {"process_start": t_proc, "torch_imported": time.time()}
     heartbeat(force=True)
@@ -669,6 +686,11 @@ def run(args) -> Dict[str, Any]:
             or getattr(adapter, "graph_error", None),
             "allreduce": getattr(getattr(adapter, "trainer", None), "allreduce_backend", "nccl" if world > 1 else "none"),
         })
+    if args.dump_outputs and n_timed > 0:
+        # collective: with the owner-sharded optimizer each rank keeps only its own range of the master weights current
+        adapter.prepare_state()
+        if rank == 0:
+            dump_outputs(args.dump_outputs, adapter, losses[-n_timed:])
     if rank == 0 and args.result:
         os.makedirs(os.path.dirname(os.path.abspath(args.result)), exist_ok=True)
         with open(args.result + ".tmp", "w") as f:
@@ -693,11 +715,13 @@ def parse_args(argv=None):
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--lr", type=float, default=3e-4)
     ap.add_argument("--seed", type=int, default=0)
-    ap.add_argument("--gemm", default="tcgen05", choices=["tcgen05", "cublas"])
+    ap.add_argument("--gemm", default="wgmma", choices=["wgmma", "cublas"])
     ap.add_argument("--no-graph", action="store_true")
     ap.add_argument("--cpu", action="store_true")
     ap.add_argument("--elastic", action="store_true")
     ap.add_argument("--result", default="")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="after the timed steps, write what they computed to DIR/*.npy (see dump_outputs)")
     ap.add_argument("--ckpt-dir", default="")
     ap.add_argument("--ckpt-every", type=int, default=0)
     ap.add_argument("--step-sleep", type=float, default=0.0)

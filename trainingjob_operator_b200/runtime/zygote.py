@@ -46,7 +46,7 @@ def _preload(cuda: bool = False) -> None:
         try:
             from trainingjob_operator_b200.ops import lib as _lib
 
-            _lib.load(build_if_missing=False)                              # dlopen + module load of the sm_100a kernels
+            _lib.load(build_if_missing=False)                              # dlopen + module load of the sm_90a kernels
         except Exception:  # noqa: BLE001
             pass
         try:

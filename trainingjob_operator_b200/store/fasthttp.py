@@ -2,7 +2,7 @@
 
 ``http.server`` and ``http.client`` parse every header block with the e-mail package (``email.feedparser``, policy
 objects, ``Message``): ~100 us per message in this interpreter, on both ends of every API call -- more than a third of the
-API-server process' CPU time under the throughput benchmark (``profiles/control_plane_throughput.json``), where that
+API-server process' CPU time under the throughput benchmark (``tools/throughput_bench.py --daemons``), where that
 process is the bottleneck of the three-daemon topology.  The headers this API needs are a handful of ``Name: value``
 lines; ``read_headers`` reads them into a case-insensitive dict, ``FastResponse`` is ``http.client.HTTPResponse`` with that
 parser, and the server's handler uses it in its own ``parse_request`` (``store/http.py``).  Semantics kept: header names
