@@ -105,13 +105,29 @@ class _LayerBufs:
 
 
 class GPT2Engine:
-    """Explicit fwd/bwd/optimizer for a fixed (B, T) micro-batch on one GPU."""
+    """Explicit fwd/bwd/optimizer for a fixed (B, T) micro-batch on one GPU.
+
+    ``doc_mask=True`` trains on packed documents: a step also reads ``doc_start`` (int32 [B*T], the sequence-local index of
+    the first token of each token's document) and a token attends only to earlier tokens of its own document.  Only the
+    wgmma attention kernels implement that mask, so they are used for the forward and the backward, and an engine they
+    cannot serve is refused at construction."""
+
+    doc_mask = False
+    doc_start = None
 
     def __init__(self, cfg: GPT2Config, batch_size: int, seq_len: int, device="cuda", seed: int = 0,
-                 gemm_backend: str = "wgmma", causal: bool = True):
+                 gemm_backend: str = "wgmma", causal: bool = True, doc_mask: bool = False):
         from ..ops import functional as F
 
         assert seq_len <= cfg.block_size and cfg.n_embd % 256 == 0
+        if doc_mask:
+            why = [w for bad, w in ((not causal, "it needs causal attention"),
+                                    (seq_len % 128, f"the sequence length {seq_len} is not a multiple of 128"),
+                                    (cfg.n_embd // cfg.n_head != 64, f"the head dim {cfg.n_embd // cfg.n_head} is not 64"),
+                                    (gemm_backend != "wgmma", f"gemm_backend is {gemm_backend!r}, not 'wgmma'")) if bad]
+            if why:
+                raise ValueError("document-masked attention runs on the wgmma attention kernels only, which cannot serve "
+                                 "this engine: " + "; ".join(why))
         self.F = F
         self.cfg = cfg
         self.B, self.T = batch_size, seq_len
@@ -127,6 +143,9 @@ class GPT2Engine:
         self.attn_bwd_impl = os.environ.get("AITJ_ATTN_BWD", "cudnn")
         if self.attn_impl != "wgmma":
             self.attn_bwd_impl = "cudnn"
+        self.doc_mask = bool(doc_mask)
+        if self.doc_mask:
+            self.attn_impl = self.attn_bwd_impl = "wgmma"
         self._attn_delta = None
         self._dq_acc = None
         self._philox = torch.zeros((), dtype=torch.int64, device=device)
@@ -143,6 +162,8 @@ class GPT2Engine:
         f32 = dict(device=self.dev, dtype=torch.float32)
         self.tok = torch.zeros(M, dtype=torch.int64, device=self.dev)
         self.tgt = torch.zeros(M, dtype=torch.int64, device=self.dev)
+        if self.doc_mask:
+            self.doc_start = torch.zeros(M, dtype=torch.int32, device=self.dev)
         self.x0 = torch.empty(M, C, **bf)
         self.layers = [_LayerBufs(M, C, self.dev) for _ in range(cfg.n_layer)]
         self.lnf = torch.empty(M, C, **bf)
@@ -183,6 +204,8 @@ class GPT2Engine:
 
     def input_tensors(self) -> List[torch.Tensor]:
         """Device tensors a step reads its inputs from, in the order the data source yields them."""
+        if self.doc_mask:
+            return [self.tok, self.tgt, self.doc_start]
         return [self.tok, self.tgt]
 
     # ------------------------------------------------------------------ GEMM front-ends
@@ -294,7 +317,10 @@ class GPT2Engine:
             # writes [B*T, H*D] and the log-sum-exp the backward needs
             if lb.lse is None:
                 lb.lse = torch.empty(B, H, T, device=self.dev, dtype=torch.float32)
-            self.F.attention_fwd(lb.qkv, lb.att, lb.lse, B, T, H, causal=self.causal)
+            if self.doc_mask:
+                self.F.attention_fwd(lb.qkv, lb.att, lb.lse, B, T, H, causal=self.causal, doc_start=self.doc_start)
+            else:
+                self.F.attention_fwd(lb.qkv, lb.att, lb.lse, B, T, H, causal=self.causal)
             lb.att_in = lb.att
             return
         qkv = lb.qkv.view(B, T, 3, H, D)
@@ -319,8 +345,12 @@ class GPT2Engine:
             if self._dq_acc is None:
                 self._attn_delta = torch.empty(B, H, T, device=self.dev, dtype=torch.float32)
                 self._dq_acc = torch.zeros(B * T, H * D, device=self.dev, dtype=torch.float32)
-            self.F.attention_bwd(lb.qkv, lb.att, d_att, lb.lse, self._attn_delta, self._dq_acc, d_qkv, B, T, H,
-                                 causal=self.causal)
+            if self.doc_mask:
+                self.F.attention_bwd(lb.qkv, lb.att, d_att, lb.lse, self._attn_delta, self._dq_acc, d_qkv, B, T, H,
+                                     causal=self.causal, doc_start=self.doc_start)
+            else:
+                self.F.attention_bwd(lb.qkv, lb.att, d_att, lb.lse, self._attn_delta, self._dq_acc, d_qkv, B, T, H,
+                                     causal=self.causal)
             self.F.colsum(d_qkv, d_bias)
             return
         do = d_att.view(B, T, H, D).transpose(1, 2)
@@ -511,17 +541,28 @@ class GPT2Reference(torch.nn.Module):
     def p(self, name: str) -> torch.Tensor:
         return self.w[name.replace(".", "_")]
 
-    def forward(self, tok: torch.Tensor, tgt: torch.Tensor) -> torch.Tensor:
+    def forward(self, tok: torch.Tensor, tgt: torch.Tensor, doc_start: torch.Tensor = None) -> torch.Tensor:
+        """``doc_start`` ([B, T] or [B*T], see ``GPT2Engine``): token q attends to key k iff doc_start[q] <= k <= q."""
         cfg = self.cfg
         B, T = tok.shape
         C, H = cfg.n_embd, cfg.n_head
+        mask = None
+        if doc_start is not None:
+            assert self.causal
+            ds = doc_start.reshape(B, 1, T, 1).long()
+            k = torch.arange(T, device=tok.device).view(1, 1, 1, T)
+            q = torch.arange(T, device=tok.device).view(1, 1, T, 1)
+            mask = (k >= ds) & (k <= q)                        # [B, 1, T, T], True = attend
         x = self.p("wte")[tok] + self.p("wpe")[:T]
         for i in range(cfg.n_layer):
             q = f"h{i}."
             h = TF.layer_norm(x, (C,), self.p(q + "ln1_w"), self.p(q + "ln1_b"))
             qkv = h @ self.p(q + "qkv_w").t() + self.p(q + "qkv_b")
             qh, kh, vh = [t.view(B, T, H, C // H).transpose(1, 2) for t in qkv.split(C, dim=-1)]
-            a = TF.scaled_dot_product_attention(qh, kh, vh, is_causal=self.causal)
+            if mask is None:
+                a = TF.scaled_dot_product_attention(qh, kh, vh, is_causal=self.causal)
+            else:
+                a = TF.scaled_dot_product_attention(qh, kh, vh, attn_mask=mask)
             a = a.transpose(1, 2).reshape(B, T, C)
             x = x + a @ self.p(q + "proj_w").t() + self.p(q + "proj_b")
             h = TF.layer_norm(x, (C,), self.p(q + "ln2_w"), self.p(q + "ln2_b"))

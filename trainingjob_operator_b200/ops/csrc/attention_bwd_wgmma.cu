@@ -9,6 +9,10 @@
 //   dQ   = dS K                                         (dS^T staged in shared memory, read as a transposed A operand)
 // and dQ is added into an fp32 scratch with red.global.add (several key blocks contribute to one query row); a last
 // pass converts it to bf16 into the packed gradient and clears the scratch.  delta = rowsum(dO * O) comes first.
+//
+// Document mask (kDoc; see attention_wgmma.cu): key k is seen by the queries q >= k with doc_start[q] <= k.  A key block
+// walks the query blocks from its own up to the one holding the last query that sees its last key, found by a binary
+// search over the (monotone) doc_start of the sequence, and P = 0 where k < doc_start[q].
 #include "ptx.cuh"
 
 namespace aitj {
@@ -26,12 +30,14 @@ struct AttnBwdArgs {
   const float* delta;   // [B, H, T]
   float* dq_acc;        // [B*T, H*64]
   __nv_bfloat16* d_qkv; // [B*T, 3*H*64]
+  const int* doc_start; // [B*T] (kDoc only)
 };
 
 __device__ __forceinline__ void red_add_v2_f32_ab(float* p, float a, float b) {
   asm volatile("red.global.add.v2.f32 [%0], {%1,%2};" ::"l"(p), "f"(a), "f"(b) : "memory");
 }
 
+template <bool kDoc>
 __global__ void __launch_bounds__(kAbThreads) attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_qkv,
                                                               const __grid_constant__ CUtensorMap tmap_do,
                                                               const AttnBwdArgs a) {
@@ -53,8 +59,22 @@ __global__ void __launch_bounds__(kAbThreads) attn_bwd_kernel(const __grid_const
   const int row0 = b * T;
   const int kv0 = kvt * AB_B;
   const int i0 = a.causal ? kvt : 0;
-  const int n_q = T / AB_B;
+  int n_q = T / AB_B;
   const int tid = threadIdx.x;
+  const int* ds_seq = kDoc ? a.doc_start + row0 : nullptr;
+  if (kDoc) {
+    // the queries past this block's last key that still see it form a prefix of (kv_last, T): those whose document
+    // starts at or before kv_last.  First index past that prefix, by binary search; then clamp the block range into
+    // [i0 + 1, T / 64] (a malformed doc_start cannot move a TMA coordinate out of this sequence)
+    const int kv_last = kv0 + AB_B - 1;
+    int lo = kv_last + 1, hi = T;
+    while (lo < hi) {
+      const int mid = (lo + hi) >> 1;
+      if (ds_seq[mid] <= kv_last) lo = mid + 1;
+      else hi = mid;
+    }
+    n_q = min(max((lo + AB_B - 1) / AB_B, i0 + 1), n_q);
+  }
 
   if (tid == 0) {
     tma_prefetch_desc(&tmap_qkv);
@@ -113,21 +133,44 @@ __global__ void __launch_bounds__(kAbThreads) attn_bwd_kernel(const __grid_const
 
     const int qb = i * AB_B;
     const bool mask = a.causal && i == kvt;        // the diagonal block: key kv0 + r sees queries >= kv0 + r only
+    // kDoc: some query of this block starts its document past this block's first key (the block's last query has the
+    // largest document start)
+    const bool dmask = kDoc && kv0 < ds_seq[qb + AB_B - 1];
+    if (dmask) {     // (a separate loop: blocks without a document boundary run the causal kernel's loop unchanged)
 #pragma unroll
-    for (int jj = 0; jj < 8; ++jj) {
-      const int qc = qb + 8 * jj + 2 * t4;
-      const float2 ls = *reinterpret_cast<const float2*>(lse + qc);
-      const float2 dl = *reinterpret_cast<const float2*>(delta + qc);
+      for (int jj = 0; jj < 8; ++jj) {
+        const int qc = qb + 8 * jj + 2 * t4;
+        const float2 ls = *reinterpret_cast<const float2*>(lse + qc);
+        const float2 dl = *reinterpret_cast<const float2*>(delta + qc);
+        const int2 dsq = *reinterpret_cast<const int2*>(ds_seq + qc);
 #pragma unroll
-      for (int hh = 0; hh < 2; ++hh)
+        for (int hh = 0; hh < 2; ++hh)
 #pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const int idx = 4 * jj + 2 * hh + e;
-          float p = fast_exp2(st[idx] * a.scale_log2 - (e ? ls.y : ls.x) * 1.4426950408889634f);
-          if (mask && 8 * jj + 2 * t4 + e < r_loc + 8 * hh) p = 0.f;
-          st[idx] = p;
-          dpt[idx] = p * (dpt[idx] - (e ? dl.y : dl.x));
-        }
+          for (int e = 0; e < 2; ++e) {
+            const int idx = 4 * jj + 2 * hh + e;
+            float p = fast_exp2(st[idx] * a.scale_log2 - (e ? ls.y : ls.x) * 1.4426950408889634f);
+            if ((mask && 8 * jj + 2 * t4 + e < r_loc + 8 * hh) || kv0 + r_loc + 8 * hh < (e ? dsq.y : dsq.x)) p = 0.f;
+            st[idx] = p;
+            dpt[idx] = p * (dpt[idx] - (e ? dl.y : dl.x));
+          }
+      }
+    } else {
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj) {
+        const int qc = qb + 8 * jj + 2 * t4;
+        const float2 ls = *reinterpret_cast<const float2*>(lse + qc);
+        const float2 dl = *reinterpret_cast<const float2*>(delta + qc);
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int idx = 4 * jj + 2 * hh + e;
+            float p = fast_exp2(st[idx] * a.scale_log2 - (e ? ls.y : ls.x) * 1.4426950408889634f);
+            if (mask && 8 * jj + 2 * t4 + e < r_loc + 8 * hh) p = 0.f;
+            st[idx] = p;
+            dpt[idx] = p * (dpt[idx] - (e ? dl.y : dl.x));
+          }
+      }
     }
     uint32_t pa[4][4], dsa[4][4];
 #pragma unroll
@@ -266,11 +309,14 @@ extern "C" {
 // qkv bf16 [B*T, 3*H*64]; out, d_out bf16 [B*T, H*64]; lse fp32 [B,H,T] (natural log, from aitj_attn_fwd);
 // delta fp32 [B,H,T] scratch; dq_acc fp32 [B*T, H*64] scratch that MUST be zero on entry (it is zero again on exit);
 // d_qkv bf16 [B*T, 3*H*64] receives dq | dk | dv.  T % 128 == 0.  scale <= 0 selects 1/sqrt(64).
+// doc_start: null, or the int32 [B*T] document starts the forward was given (causal only).
 int aitj_attn_bwd(const void* qkv, const void* out, const void* d_out, const void* lse, void* delta, void* dq_acc,
-                  void* d_qkv, int B, int T, int H, int causal, float scale, void* stream_ptr) {
+                  void* d_qkv, const void* doc_start, int B, int T, int H, int causal, float scale, void* stream_ptr) {
   using namespace aitj;
   if (B <= 0 || T <= 0 || H <= 0) return 0;
   if (T % 128) return -1;
+  if (doc_start && !causal) return -5;
+  if (reinterpret_cast<uintptr_t>(doc_start) & 7) return -4;   // read as int2 pairs
   const int C = H * AB_D;
   const uint64_t rows = static_cast<uint64_t>(B) * T;
   CUtensorMap tq, tdo;
@@ -287,12 +333,15 @@ int aitj_attn_bwd(const void* qkv, const void* out, const void* d_out, const voi
   a.delta = reinterpret_cast<const float*>(delta);
   a.dq_acc = reinterpret_cast<float*>(dq_acc);
   a.d_qkv = reinterpret_cast<__nv_bfloat16*>(d_qkv);
+  a.doc_start = reinterpret_cast<const int*>(doc_start);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_ptr);
   constexpr int kSmem = 57344 + 1024 + 64;
-  static bool configured = false;
-  if (!configured) {
-    if (cudaFuncSetAttribute(attn_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem) != cudaSuccess) return -20;
-    configured = true;
+  static bool configured[2] = {false, false};
+  const int v = doc_start ? 1 : 0;
+  if (!configured[v]) {
+    if (cudaFuncSetAttribute(v ? attn_bwd_kernel<true> : attn_bwd_kernel<false>,
+                             cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem) != cudaSuccess) return -20;
+    configured[v] = true;
   }
   static int n_sms = 0;
   if (!n_sms) {
@@ -305,7 +354,10 @@ int aitj_attn_bwd(const void* qkv, const void* out, const void* d_out, const voi
   if (blocks > n_sms * 8) blocks = n_sms * 8;
   attn_delta_kernel<<<blocks, 256, 0, st>>>(reinterpret_cast<const __nv_bfloat16*>(d_out),
                                             reinterpret_cast<const __nv_bfloat16*>(out), reinterpret_cast<float*>(delta), B, T, H);
-  attn_bwd_kernel<<<dim3(T / AB_B, B * H), kAbThreads, kSmem, st>>>(tq, tdo, a);
+  if (v)
+    attn_bwd_kernel<true><<<dim3(T / AB_B, B * H), kAbThreads, kSmem, st>>>(tq, tdo, a);
+  else
+    attn_bwd_kernel<false><<<dim3(T / AB_B, B * H), kAbThreads, kSmem, st>>>(tq, tdo, a);
   const size_t nvec = rows * (C / 8);
   blocks = static_cast<int>((nvec + 255) / 256);
   if (blocks > n_sms * 8) blocks = n_sms * 8;

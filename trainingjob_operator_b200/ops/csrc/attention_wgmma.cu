@@ -7,6 +7,11 @@
 // each, double-buffered, the next block's TMA load in flight while the current one is used).  P never leaves the
 // registers: the fp32 S fragment of a warpgroup has the row / column layout of a wgmma A operand, so P is packed to
 // bf16 in place and multiplied with V (read transposed from shared memory: V is stored key-major).
+//
+// Document mask (kDoc, packed sequences): doc_start[b*T + t] is the sequence-local index of the first token of the
+// document holding token t (non-decreasing along the sequence, 0 at t = 0); query q sees key k iff
+// doc_start[q] <= k <= q.  A tile's key loop starts at the block of its first row's document start instead of block 0,
+// so with short documents most key blocks are never loaded.
 #include "ptx.cuh"
 
 namespace aitj {
@@ -22,8 +27,10 @@ struct AttnArgs {
   float scale_log2;   // softmax scale * log2(e)
   float* lse;         // [B, H, T] natural-log sum-exp of the scaled scores (what the backward needs)
   __nv_bfloat16* out; // [B*T, H*64]
+  const int* doc_start; // [B*T] (kDoc only)
 };
 
+template <bool kDoc>
 __global__ void __launch_bounds__(kAttThreads) attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_qkv,
                                                                const AttnArgs a) {
   extern __shared__ uint8_t smem_raw[];
@@ -43,6 +50,9 @@ __global__ void __launch_bounds__(kAttThreads) attn_fwd_kernel(const __grid_cons
   const int q0 = qt * ATT_BM;
   const int n_kv = a.causal ? (q0 + ATT_BM) / ATT_BN : T / ATT_BN;
   const int tid = threadIdx.x;
+  // first key block: the one holding the document start of the tile's first row (the smallest in the tile), clamped
+  // into [0, q0] so that a malformed doc_start cannot move a TMA coordinate out of this sequence
+  const int j0 = kDoc ? min(max(a.doc_start[row0 + q0], 0), q0) / ATT_BN : 0;
 
   if (tid == 0) {
     tma_prefetch_desc(&tmap_qkv);
@@ -57,8 +67,8 @@ __global__ void __launch_bounds__(kAttThreads) attn_fwd_kernel(const __grid_cons
     tma_load_2d(sq, &tmap_qkv, q_full, h * ATT_D, row0 + q0);
     tma_load_2d(sq + 8192, &tmap_qkv, q_full, h * ATT_D, row0 + q0 + 64);
     mbar_arrive_expect_tx(&kv_full[0], 16384);
-    tma_load_2d(sk, &tmap_qkv, &kv_full[0], (H + h) * ATT_D, row0);
-    tma_load_2d(sv, &tmap_qkv, &kv_full[0], (2 * H + h) * ATT_D, row0);
+    tma_load_2d(sk, &tmap_qkv, &kv_full[0], (H + h) * ATT_D, row0 + j0 * ATT_BN);
+    tma_load_2d(sv, &tmap_qkv, &kv_full[0], (2 * H + h) * ATT_D, row0 + j0 * ATT_BN);
   }
 
   const int wg = tid >> 7;
@@ -66,6 +76,14 @@ __global__ void __launch_bounds__(kAttThreads) attn_fwd_kernel(const __grid_cons
   const int lane = tid & 31;
   const int t4 = lane & 3;
   const int qrow = q0 + wg * 64 + wl * 16 + (lane >> 2);   // this thread's rows: qrow and qrow + 8 (sequence positions)
+  // kDoc: the document starts of this thread's two rows, and the largest one of the warpgroup's 64 rows (its last row's):
+  // key blocks that start at or past it need only the causal mask
+  int ds[2] = {0, 0}, ds_hi = 0;
+  if (kDoc) {
+    ds[0] = min(max(a.doc_start[row0 + qrow], 0), qrow);
+    ds[1] = min(max(a.doc_start[row0 + qrow + 8], 0), qrow + 8);
+    ds_hi = a.doc_start[row0 + q0 + wg * 64 + 63];
+  }
   float o[32];
 #pragma unroll
   for (int i = 0; i < 32; ++i) o[i] = 0.f;
@@ -73,15 +91,16 @@ __global__ void __launch_bounds__(kAttThreads) attn_fwd_kernel(const __grid_cons
   const uint32_t q_addr = smem_u32(sq) + wg * 8192;
 
   mbar_wait(q_full, 0);
-  for (int j = 0; j < n_kv; ++j) {
-    const int buf = j & 1;
+  for (int j = j0; j < n_kv; ++j) {
+    const int it = j - j0;
+    const int buf = it & 1;
     if (tid == 0 && j + 1 < n_kv) {
       // the other buffer was last read in iteration j-1, which every thread has left (barrier at its end)
       mbar_arrive_expect_tx(&kv_full[buf ^ 1], 16384);
       tma_load_2d(sk + (buf ^ 1) * 8192, &tmap_qkv, &kv_full[buf ^ 1], (H + h) * ATT_D, row0 + (j + 1) * ATT_BN);
       tma_load_2d(sv + (buf ^ 1) * 8192, &tmap_qkv, &kv_full[buf ^ 1], (2 * H + h) * ATT_D, row0 + (j + 1) * ATT_BN);
     }
-    mbar_wait(&kv_full[buf], (j >> 1) & 1);
+    mbar_wait(&kv_full[buf], (it >> 1) & 1);
     const uint32_t k_addr = smem_u32(sk) + buf * 8192;
     const uint32_t v_addr = smem_u32(sv) + buf * 8192;
     float s[32];
@@ -96,33 +115,58 @@ __global__ void __launch_bounds__(kAttThreads) attn_fwd_kernel(const __grid_cons
 
     const int kv0 = j * ATT_BN;
     const bool mask = a.causal && kv0 + ATT_BN - 1 > q0 + wg * 64;
+    const bool dmask = kDoc && kv0 < ds_hi;
     float mx[2] = {-INFINITY, -INFINITY};
+    if (dmask) {     // (a separate loop: blocks without a document boundary run the causal kernel's loop unchanged)
 #pragma unroll
-    for (int jj = 0; jj < 8; ++jj)
+      for (int jj = 0; jj < 8; ++jj)
 #pragma unroll
-      for (int hh = 0; hh < 2; ++hh)
+        for (int hh = 0; hh < 2; ++hh)
 #pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const int idx = 4 * jj + 2 * hh + e;
-          float v = s[idx] * a.scale_log2;
-          if (mask && kv0 + 8 * jj + 2 * t4 + e > qrow + 8 * hh) v = -INFINITY;
-          s[idx] = v;
-          mx[hh] = fmaxf(mx[hh], v);
-        }
-    float alpha[2], ls[2] = {0.f, 0.f};
+          for (int e = 0; e < 2; ++e) {
+            const int idx = 4 * jj + 2 * hh + e;
+            const int k = kv0 + 8 * jj + 2 * t4 + e;
+            float v = s[idx] * a.scale_log2;
+            if ((mask && k > qrow + 8 * hh) || k < ds[hh]) v = -INFINITY;
+            s[idx] = v;
+            mx[hh] = fmaxf(mx[hh], v);
+          }
+    } else {
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int idx = 4 * jj + 2 * hh + e;
+            float v = s[idx] * a.scale_log2;
+            if (mask && kv0 + 8 * jj + 2 * t4 + e > qrow + 8 * hh) v = -INFINITY;
+            s[idx] = v;
+            mx[hh] = fmaxf(mx[hh], v);
+          }
+    }
+    float alpha[2], m_sub[2], ls[2] = {0.f, 0.f};
 #pragma unroll
     for (int hh = 0; hh < 2; ++hh) {
       mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 1));
       mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 2));
-      // key 0 is visible to every query row and comes in block 0, so m is finite from then on
+      // without a document mask key 0 is visible to every query row and comes in block 0, so m is finite from then
+      // on.  With one, a row whose document starts past this block has seen nothing but -inf yet: it keeps alpha = 1
+      // and gets p = 0 (subtracting 0 instead of -inf), never exp2(-inf - -inf)
       const float m_new = fmaxf(m[hh], mx[hh]);
-      alpha[hh] = fast_exp2(m[hh] - m_new);
+      if (kDoc && m_new == -INFINITY) {
+        alpha[hh] = 1.f;
+        m_sub[hh] = 0.f;
+      } else {
+        alpha[hh] = fast_exp2(m[hh] - m_new);
+        m_sub[hh] = m_new;
+      }
       m[hh] = m_new;
     }
 #pragma unroll
     for (int idx = 0; idx < 32; ++idx) {
       const int hh = (idx >> 1) & 1;
-      const float p = fast_exp2(s[idx] - m[hh]);
+      const float p = fast_exp2(s[idx] - m_sub[hh]);
       s[idx] = p;
       ls[hh] += p;
       o[idx] *= alpha[hh];
@@ -190,10 +234,14 @@ extern "C" {
 
 // qkv: bf16 [B*T, 3*H*64] (q | k | v, heads contiguous inside each third);  out: bf16 [B*T, H*64];
 // lse: fp32 [B, H, T].  T must be a multiple of 128.  scale <= 0 selects 1/sqrt(64).
-int aitj_attn_fwd(const void* qkv, void* out, void* lse, int B, int T, int H, int causal, float scale, void* stream_ptr) {
+// doc_start: null, or int32 [B*T] document starts (see the top of this file; causal only).
+int aitj_attn_fwd(const void* qkv, void* out, void* lse, const void* doc_start, int B, int T, int H, int causal,
+                  float scale, void* stream_ptr) {
   using namespace aitj;
   if (B <= 0 || T <= 0 || H <= 0) return 0;
   if (T % ATT_BM) return -1;
+  if (doc_start && !causal) return -5;
+  if (reinterpret_cast<uintptr_t>(doc_start) & 7) return -4;   // read as int2 pairs
   if ((reinterpret_cast<uintptr_t>(qkv) & 15) || (reinterpret_cast<uintptr_t>(out) & 15)) return -4;
   const int C = H * ATT_D;
   CUtensorMap tq;
@@ -205,15 +253,22 @@ int aitj_attn_fwd(const void* qkv, void* out, void* lse, int B, int T, int H, in
   a.scale_log2 = scale * 1.4426950408889634f;
   a.lse = reinterpret_cast<float*>(lse);
   a.out = reinterpret_cast<__nv_bfloat16*>(out);
+  a.doc_start = reinterpret_cast<const int*>(doc_start);
   constexpr int kSmem = 49152 + 1024 + 64;
-  static bool configured = false;
-  if (!configured) {
-    if (cudaFuncSetAttribute(attn_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem) != cudaSuccess)
+  static bool configured[2] = {false, false};
+  const int v = doc_start ? 1 : 0;
+  if (!configured[v]) {
+    if (cudaFuncSetAttribute(v ? attn_fwd_kernel<true> : attn_fwd_kernel<false>,
+                             cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem) != cudaSuccess)
       return -20;
-    configured = true;
+    configured[v] = true;
   }
   dim3 grid(T / ATT_BM, B * H);
-  attn_fwd_kernel<<<grid, kAttThreads, kSmem, reinterpret_cast<cudaStream_t>(stream_ptr)>>>(tq, a);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_ptr);
+  if (v)
+    attn_fwd_kernel<true><<<grid, kAttThreads, kSmem, st>>>(tq, a);
+  else
+    attn_fwd_kernel<false><<<grid, kAttThreads, kSmem, st>>>(tq, a);
   return cudaPeekAtLastError() == cudaSuccess ? 0 : -30;
 }
 

@@ -224,27 +224,46 @@ def colsum(dy, db):
     lib.call("aitj_colsum", dy.data_ptr(), db.data_ptr(), M, N, _is_mc(db), _stream())
 
 
-def attention_fwd(qkv, out, lse, B, T, H, causal=True, scale=0.0):
+def _check_doc_start(doc_start, B, T, causal):
+    """``doc_start``: int32 [B*T], the sequence-local index of the first token of the document holding each token; query
+    q then sees key k iff doc_start[q] <= k <= q.  Only a causal attention takes one."""
+    if doc_start is None:
+        return None
+    if not causal:
+        raise ValueError("a document mask needs causal attention")
+    if doc_start.dtype != torch.int32 or not doc_start.is_contiguous() or doc_start.numel() != B * T:
+        raise ValueError(f"doc_start must be a contiguous int32 tensor of {B * T} elements, got "
+                         f"{doc_start.dtype} {tuple(doc_start.shape)}")
+    if doc_start.data_ptr() % 8:
+        raise ValueError("doc_start must be 8-byte aligned (the kernels read it in pairs)")
+    return doc_start.data_ptr()
+
+
+def attention_fwd(qkv, out, lse, B, T, H, causal=True, scale=0.0, doc_start=None):
     """Flash attention forward on wgmma (head dim 64): qkv bf16 [B*T, 3*H*64] packed q|k|v -> out bf16 [B*T, H*64],
-    lse fp32 [B, H, T] (natural-log sum-exp of the scaled scores).  T % 128 == 0."""
+    lse fp32 [B, H, T] (natural-log sum-exp of the scaled scores).  T % 128 == 0.  ``doc_start`` (int32 [B*T], causal
+    only): document mask of packed sequences, see ``_check_doc_start``."""
     assert qkv.dtype == torch.bfloat16 and out.dtype == torch.bfloat16 and lse.dtype == torch.float32
     assert qkv.is_contiguous() and out.is_contiguous() and lse.is_contiguous()
     assert qkv.shape == (B * T, 3 * H * 64) and out.shape == (B * T, H * 64) and lse.numel() == B * H * T
-    lib.call("aitj_attn_fwd", qkv.data_ptr(), out.data_ptr(), lse.data_ptr(), B, T, H, int(causal), float(scale),
+    ds = _check_doc_start(doc_start, B, T, causal)
+    lib.call("aitj_attn_fwd", qkv.data_ptr(), out.data_ptr(), lse.data_ptr(), ds, B, T, H, int(causal), float(scale),
              _stream())
     return out
 
 
-def attention_bwd(qkv, out, d_out, lse, delta, dq_acc, d_qkv, B, T, H, causal=True, scale=0.0):
+def attention_bwd(qkv, out, d_out, lse, delta, dq_acc, d_qkv, B, T, H, causal=True, scale=0.0, doc_start=None):
     """Flash attention backward on wgmma (head dim 64).  qkv / d_qkv bf16 [B*T, 3*H*64] (d_qkv receives dq | dk | dv in
     place), out / d_out bf16 [B*T, H*64], lse fp32 [B,H,T] from ``attention_fwd``; delta fp32 [B,H,T] and dq_acc fp32
-    [B*T, H*64] are scratch -- dq_acc must be zero on entry and is zero again on exit."""
+    [B*T, H*64] are scratch -- dq_acc must be zero on entry and is zero again on exit.  ``doc_start``: the document mask
+    the forward was given."""
     assert qkv.dtype == torch.bfloat16 and d_qkv.dtype == torch.bfloat16 and dq_acc.dtype == torch.float32
     assert qkv.is_contiguous() and out.is_contiguous() and d_out.is_contiguous() and d_qkv.is_contiguous()
     assert qkv.shape == (B * T, 3 * H * 64) and d_qkv.shape == qkv.shape and out.shape == (B * T, H * 64)
     assert d_out.shape == out.shape and dq_acc.shape == out.shape and lse.numel() == B * H * T == delta.numel()
+    ds = _check_doc_start(doc_start, B, T, causal)
     lib.call("aitj_attn_bwd", qkv.data_ptr(), out.data_ptr(), d_out.data_ptr(), lse.data_ptr(), delta.data_ptr(),
-             dq_acc.data_ptr(), d_qkv.data_ptr(), B, T, H, int(causal), float(scale), _stream())
+             dq_acc.data_ptr(), d_qkv.data_ptr(), ds, B, T, H, int(causal), float(scale), _stream())
     lib.LAUNCHES += 2          # delta + dq_finish ride along with the main kernel
     return d_qkv
 

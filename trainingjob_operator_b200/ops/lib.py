@@ -61,8 +61,8 @@ _F = ctypes.c_float
 _SIGS = {
     "aitj_gemm_bf16": [_P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _P, _P, _P, _I, _I, _I, _I, _P],
     "aitj_num_sms": [],
-    "aitj_attn_fwd": [_P, _P, _P, _I, _I, _I, _I, _F, _P],
-    "aitj_attn_bwd": [_P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _F, _P],
+    "aitj_attn_fwd": [_P, _P, _P, _P, _I, _I, _I, _I, _F, _P],
+    "aitj_attn_bwd": [_P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _F, _P],
     "aitj_gemm_set_colsum": [_P],
     "aitj_layernorm_fwd": [_P, _P, _P, _P, _P, _P, _I, _I, _F, _P],
     "aitj_layernorm_bwd": [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _P],

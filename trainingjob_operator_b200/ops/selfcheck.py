@@ -600,8 +600,196 @@ def case_attention():
     return ok
 
 
+# ----------------------------------------------------------------------------- document-masked attention
+def doc_start_from_lengths(lengths, T):
+    """int32 [T] document starts of one sequence cut into documents of the given lengths (cycled until T is filled)."""
+    ds, pos, i = [], 0, 0
+    while pos < T:
+        n = min(lengths[i % len(lengths)], T - pos)
+        ds += [pos] * n
+        pos += n
+        i += 1
+    return torch.tensor(ds, dtype=torch.int32)
+
+
+def _doc_mask_ref(qkv, d_out, B, T, H, doc_start):
+    """fp32 attention with the explicit boolean document mask: out, lse, and dq / dk / dv for ``d_out``."""
+    q, k, v = (qkv.view(B, T, 3, H, 64)[:, :, i].transpose(1, 2).float().requires_grad_(True) for i in range(3))
+    ds = doc_start.view(B, 1, T, 1).long()
+    kk = torch.arange(T, device=qkv.device).view(1, 1, 1, T)
+    qq = torch.arange(T, device=qkv.device).view(1, 1, T, 1)
+    allowed = (kk >= ds) & (kk <= qq)
+    s = ((q @ k.transpose(-1, -2)) * 0.125).masked_fill(~allowed, float("-inf"))
+    o = torch.softmax(s, -1) @ v
+    grads = torch.autograd.grad(o, (q, k, v), d_out.view(B, T, H, 64).transpose(1, 2).float())
+    return (o.detach().transpose(1, 2).reshape(B * T, H * 64), torch.logsumexp(s.detach(), -1), grads)
+
+
+def _run_attn(qkv, d_out, B, T, H, doc_start):
+    C = H * 64
+    out = torch.empty(B * T, C, device="cuda", dtype=torch.bfloat16)
+    lse = torch.empty(B, H, T, device="cuda")
+    F.attention_fwd(qkv, out, lse, B, T, H, causal=True, doc_start=doc_start)
+    delta = torch.empty(B, H, T, device="cuda")
+    dq_acc = torch.zeros(B * T, C, device="cuda")
+    d_qkv = torch.full_like(qkv, float("nan"))
+    F.attention_bwd(qkv, out, d_out, lse, delta, dq_acc, d_qkv, B, T, H, causal=True, doc_start=doc_start)
+    torch.cuda.synchronize()
+    return out, lse, d_qkv, dq_acc
+
+
+def case_attention_docs():
+    """Document-masked wgmma attention forward and backward vs an fp32 reference with an explicit boolean mask, on
+    layouts that put document boundaries everywhere a block edge could go wrong; one document per row against the
+    unmasked causal kernels; every token its own document."""
+    ok = True
+    mixed = [1, 63, 64, 65, 127, 128, 129]
+    layouts = [
+        (1, 128, 1, [[1, 63, 64]]),
+        (1, 256, 3, [mixed]),
+        (1, 1024, 12, [mixed]),
+        (1, 256, 1, [[127, 129]]),                     # a document starting at the last row of the first 128-row tile
+        (2, 256, 3, [[255, 1], [64, 64, 1, 127]]),     # ... and of the second; B = 2 with a different layout per row
+        (2, 1024, 3, [mixed[::-1], [300, 700, 24]]),
+        (1, 128, 3, [[1]]),                            # every token its own document
+    ]
+    for B, T, H, per_row in layouts:
+        ds = torch.cat([doc_start_from_lengths(per_row[b % len(per_row)], T) for b in range(B)]).cuda()
+        C = H * 64
+        qkv = _rand(B * T, 3 * C)
+        d_out = _rand(B * T, C)
+        out, lse, d_qkv, dq_acc = _run_attn(qkv, d_out, B, T, H, ds)
+        ref_o, ref_lse, (gq, gk, gv) = _doc_mask_ref(qkv, d_out, B, T, H, ds)
+        tag = f"B{B} T{T} H{H} docs={per_row}"[:80]
+        ok &= _check(f"doc attn fwd out {tag}", out, ref_o, 2e-2, atol_scale=5e-2)
+        ok &= _check(f"doc attn fwd lse {tag}", lse, ref_lse, 1e-3)
+        got = d_qkv.view(B, T, 3, H, 64)
+        for name, i, g in (("dq", 0, gq), ("dk", 1, gk), ("dv", 2, gv)):
+            if per_row == [[1]] and i < 2:
+                # a row that sees only itself has P = 1 and o = v, so dS = P (dP - delta) is exactly 0: dq and dk are 0 up
+                # to the rounding of dP and delta (dO . v in the tensor cores vs dO . bf16(o)), against O(1) gradients
+                worst = float(got[:, :, i].abs().max())
+                print(f"  own-document rows: |{name}| <= {worst:.2e} (exactly 0 in exact arithmetic)")
+                ok &= worst < 1e-5
+                continue
+            ok &= _check(f"doc attn bwd {name} {tag}", got[:, :, i].transpose(1, 2), g, 2e-2, rtol=5e-2,
+                         atol_scale=1.5e-1)
+        ok &= float(dq_acc.abs().max()) == 0.0
+        if per_row == [[1]]:
+            # each row attends to itself only: out is that row's v, lse its own scaled score
+            v = qkv.view(B, T, 3, H, 64)[:, :, 2].reshape(B * T, C)
+            same = bool(torch.equal(out, v))
+            print(f"  own-document rows: out == v bit for bit: {same}")
+            ok &= same
+            q, k = (qkv.view(B, T, 3, H, 64)[:, :, i].float() for i in range(2))
+            ok &= _check("own-document lse = own scaled score", lse, ((q * k).sum(-1) * 0.125).permute(0, 2, 1), 1e-4)
+    # one document per row: the masked kernels visit the same blocks in the same order as the causal ones
+    B, T, H = 2, 1024, 12
+    qkv = _rand(B * T, 3 * H * 64)
+    d_out = _rand(B * T, H * 64)
+    ref = _run_attn(qkv, d_out, B, T, H, None)
+    got = _run_attn(qkv, d_out, B, T, H, torch.zeros(B * T, dtype=torch.int32, device="cuda"))
+    for name, a, b in (("out", got[0], ref[0]), ("lse", got[1], ref[1]),
+                       ("dk", got[2].view(B * T, 3, -1)[:, 1], ref[2].view(B * T, 3, -1)[:, 1]),
+                       ("dv", got[2].view(B * T, 3, -1)[:, 2], ref[2].view(B * T, 3, -1)[:, 2])):
+        same = bool(torch.equal(a, b))
+        print(f"  one document per row vs causal kernel: {name} bit-identical: {same}")
+        ok &= same
+    # dq is summed over key blocks with fp32 atomics, whose order differs from run to run in either kernel
+    dq_g, dq_r = got[2].view(B * T, 3, -1)[:, 0], ref[2].view(B * T, 3, -1)[:, 0]
+    ok &= _check("one document per row vs causal kernel: dq (atomic order)", dq_g, dq_r, 1e-3, rtol=1e-2,
+                 atol_scale=1e-2)
+    # unsupported: a mask with full (non-causal) attention is refused by the entry point and by the kernel
+    try:
+        F.attention_fwd(qkv, got[0], got[1], B, T, H, causal=False, doc_start=torch.zeros(B * T, dtype=torch.int32,
+                                                                                          device="cuda"))
+        ok = False
+    except ValueError:
+        pass
+    rc = F.lib.load().aitj_attn_fwd(qkv.data_ptr(), got[0].data_ptr(), got[1].data_ptr(), got[1].data_ptr(), B, T, H,
+                                    0, 0.0, torch.cuda.current_stream().cuda_stream)
+    ok &= rc == -5
+    return ok
+
+
+def _doc_tokens(B, T, vocab, eot, lengths, seed):
+    """Token ids with documents of the given lengths (each opened by ``eot``, as in llm.c shards)."""
+    g = torch.Generator().manual_seed(seed)
+    tok = torch.randint(0, vocab - 1, (B, T), generator=g)
+    tok[tok == eot] = 0
+    ds = torch.stack([doc_start_from_lengths(lengths[b % len(lengths)], T) for b in range(B)])
+    starts = ds == torch.arange(T)
+    starts[:, 0] = False
+    tok[starts] = eot
+    return tok, ds
+
+
+def case_gpt2_docs():
+    """GPT2Engine(doc_mask=True) vs GPT2Reference with the same boolean document mask (loss, gradients), and documents
+    that cannot see each other: changing one document leaves every per-token loss of the others bit-identical."""
+    from ..models.gpt2 import GPT2Config, GPT2Engine, GPT2Reference
+
+    ok = True
+    cfg = GPT2Config(vocab_size=1000, n_layer=2, n_head=4, n_embd=256, block_size=256, name="t")
+    B, T, eot = 4, 256, 999
+    eng = GPT2Engine(cfg, B, T, "cuda", seed=3, doc_mask=True)
+    assert eng.attn_impl == "wgmma" and eng.attn_bwd_impl == "wgmma"
+    ref = GPT2Reference(cfg, eng.params).cuda()
+    tok, ds = _doc_tokens(B, T, cfg.vocab_size, eot, [[40, 1, 100, 115], [256], [7, 64, 129, 56], [1]], 5)
+    tok, ds = tok.cuda(), ds.cuda()
+    tgt = torch.roll(tok, -1, dims=1)
+    for dst, src in zip(eng.input_tensors(), (tok, tgt, ds)):
+        dst.copy_(src.reshape(-1))
+    eng.params.g32.zero_()
+    eng.forward(); eng.backward()
+    torch.cuda.synchronize()
+    rl = ref(tok, tgt, ds)
+    rl.backward()
+    ok &= _check("[doc_mask] loss", eng.loss, rl.detach().reshape(1), 5e-3)
+    for name in ("wte", "wpe", "h0.qkv_w", "h0.qkv_b", "h0.proj_w", "h0.fc_w", "h0.fc_b", "h0.fc2_w", "h1.ln1_w",
+                 "h1.ln2_b", "h1.fc2_w", "lnf_w", "lnf_b"):
+        ok &= _check(f"[doc_mask] grad {name}", eng.params.grad(name), ref.p(name).grad, 4e-2, rtol=1e-1,
+                     atol_scale=2.5e-1)
+    # isolation: row 0's third document ([41, 141)) gets new tokens (its end-of-text opener stays)
+    for masked in (True, False):
+        e = eng if masked else GPT2Engine(cfg, B, T, "cuda", seed=3)
+        losses = []
+        for variant in range(2):
+            t = tok.clone()
+            if variant:
+                t[0, 42:141] = (t[0, 42:141] + 17) % (cfg.vocab_size - 1)
+            ins = (t, torch.roll(t, -1, dims=1), ds)
+            for dst, src in zip(e.input_tensors(), ins):
+                dst.copy_(src.reshape(-1))
+            e.forward()
+            torch.cuda.synchronize()
+            losses.append(e.losses.view(B, T).clone())
+        others = torch.ones(B, T, dtype=torch.bool, device="cuda")
+        others[0, 41:141] = False
+        same = bool(torch.equal(losses[0][others], losses[1][others]))
+        later_changed = not torch.equal(losses[0][0, 141:], losses[1][0, 141:])
+        print(f"  doc_mask={masked}: losses of the other documents bit-identical after changing one: {same}; "
+              f"later documents of that row changed: {later_changed}")
+        ok &= same if masked else later_changed
+    # three optimizer steps reduce the loss
+    for dst, src in zip(eng.input_tensors(), (tok, tgt, ds)):
+        dst.copy_(src.reshape(-1))
+    eng.params.g32.zero_()
+    eng.forward(); eng.backward()
+    l0 = float(eng.loss.item())
+    for step in range(1, 4):
+        eng.optimizer_step(lr=1e-3, step=step)
+        eng.forward(); eng.backward()
+    l1 = float(eng.loss.item())
+    print(f"  [doc_mask] loss {l0:.4f} -> {l1:.4f}")
+    ok &= l1 < l0
+    return ok
+
+
 CASES = {
     "attention": case_attention,
+    "attention_docs": case_attention_docs,
+    "gpt2_docs": case_gpt2_docs,
     "gemm_2cta": case_gemm_2cta,
     "gemm_quad": case_gemm_quad,
     "graph_step": case_graph_step,

@@ -192,8 +192,9 @@ def sync_state(adapter, loop_step: int, device: torch.device, have_state: bool =
     """Hand-off after every (re-)rendezvous.  The source is elected, not assumed to be rank 0: the rank holding the most
     optimizer steps wins (ties: the lowest rank; ranks that only have a throw-away warm-up state bid -1), so when rank 0
     itself was the replica that got replaced, its replacement receives the survivors' state instead of overwriting it.
-    The source broadcasts {optimizer step, loop step} and then the flat state tensors.  Same call sequence on every
-    rank."""
+    The source broadcasts {optimizer step, loop step, data position} and then the flat state tensors.  Same call sequence
+    on every rank.  The data position (samples of a token corpus the job has consumed) is taken from adapters that keep
+    one and given to them; others send 0."""
     if not dist.is_initialized() or dist.get_world_size() <= 1:
         return loop_step
     from ..parallel.ddp import broadcast_state
@@ -205,11 +206,14 @@ def sync_state(adapter, loop_step: int, device: torch.device, have_state: bool =
     dist.all_reduce(bid, op=dist.ReduceOp.MAX)
     best = int(bid[0])
     src = 0 if best < 0 else world - 1 - (best % world)
-    st = torch.tensor([adapter.step_count, loop_step], dtype=torch.int64, device=cdev)
+    st = torch.tensor([adapter.step_count, loop_step, int(getattr(adapter, "data_position", 0))], dtype=torch.int64,
+                      device=cdev)
     dist.broadcast(st, src)
     broadcast_state(adapter.state_tensors(), src)
     adapter.after_state_load()
     adapter.step_count = int(st[0])
+    if hasattr(adapter, "data_position"):
+        adapter.data_position = int(st[2])
     return int(st[1])
 
 

@@ -64,17 +64,30 @@ class EngineAdapter:
             else:
                 raise ValueError(name)
             seq = min(seq, cfg.block_size)
-            self.engine = GPT2Engine(cfg, batch, seq, device, seed=args.seed, gemm_backend=args.gemm, causal=True)
-            self.data = SyntheticTokens(cfg.vocab_size, batch, seq, n_batches=4, seed=args.seed + 1)
+            doc_mask = bool(getattr(args, "doc_mask", False))
+            self.engine = GPT2Engine(cfg, batch, seq, device, seed=args.seed, gemm_backend=args.gemm, causal=True,
+                                     doc_mask=doc_mask)
+            if getattr(args, "data", ""):
+                from .data import TokenFileData
+
+                # samples consumed by the whole job; rank r of W reads [pos + r*B, pos + (r+1)*B) at a step
+                self.data_position = 0
+                self.data = TokenFileData(args.data, seq, cfg.vocab_size, doc_mask=doc_mask, eot=args.eot_token,
+                                          pin=device != "cpu")
+            else:
+                self.data = SyntheticTokens(cfg.vocab_size, batch, seq, n_batches=4, seed=args.seed + 1)
             self.flops_per_step = flops_per_token(cfg, seq) * batch * seq
         self.cfg = cfg
         self.batch, self.seq = batch, seq
-        self.h2d_bytes = self.data.bytes_per_step
+        self.h2d_bytes = self.data.bytes_per_sample * batch if hasattr(self, "data_position") else \
+            self.data.bytes_per_step
         self.d2h_bytes = 4
         self.trainer: Optional[EngineTrainer] = None
         self.args = args
         self.describe = {"model": cfg.name, "seq_len": seq, "params": self.engine.num_parameters(),
                          "gemm": args.gemm}
+        if hasattr(self, "data_position"):
+            self.describe.update(data=args.data, doc_mask=self.engine.doc_mask, windows=self.data.n_windows)
 
     def bind(self, group=None) -> None:
         old = self.trainer
@@ -87,7 +100,14 @@ class EngineAdapter:
             self.trainer.step_count = old.step_count
 
     def train_step(self) -> float:
-        return self.trainer.step(*self.data.next())
+        if not hasattr(self, "data_position"):
+            return self.trainer.step(*self.data.next())
+        world, rank = self.trainer.world, self.trainer.rank
+        host = self.data.stage(self.data_position + rank * self.batch, self.batch)
+        loss = self.trainer.step(*host)
+        self.data.in_flight()
+        self.data_position += world * self.batch     # not reached when the step fails: a discarded step reads again
+        return loss
 
     def discard_step(self) -> None:
         self.engine.params.g32.zero_()
@@ -314,7 +334,8 @@ def checkpointer(args):
 def save_checkpoint(args, adapter, step: int) -> None:
     """Snapshot the state in stream order and write it in the background; ``AITJ_CKPT_ASYNC=0`` waits for the file."""
     w = checkpointer(args)
-    w.save(step, adapter.state_tensors())
+    extra = {"data_position": int(adapter.data_position)} if hasattr(adapter, "data_position") else None
+    w.save(step, adapter.state_tensors(), extra=extra)
     if os.environ.get("AITJ_CKPT_ASYNC", "1") == "0":
         w.wait()
 
@@ -328,6 +349,8 @@ def load_checkpoint(args, adapter) -> int:
     if meta is None:
         return 0
     adapter.after_state_load()
+    if hasattr(adapter, "data_position"):
+        adapter.data_position = int(meta.get("data_position", 0))
     return int(meta["step"])
 
 
@@ -429,7 +452,8 @@ def run(args) -> Dict[str, Any]:
     if restart_count > 0 and args.ckpt_every > 0:
         start_step = load_checkpoint(args, adapter)
         adapter.step_count = start_step
-        print(f"[worker {rank}] restart #{restart_count}: resumed from checkpoint at step {start_step}", flush=True)
+        print(f"[worker {rank}] restart #{restart_count}: resumed from checkpoint at step {start_step}"
+              + (f", data position {adapter.data_position}" if hasattr(adapter, "data_position") else ""), flush=True)
     # a joiner without a checkpoint only has its throw-away warm-up state: it must never be elected as the source
     joined_step = sync_state(adapter, start_step, device, have_state=not joiner or start_step > 0)
     if joiner:
@@ -647,6 +671,8 @@ def run(args) -> Dict[str, Any]:
     result: Dict[str, Any] = {"rank": rank, "world": world, "steps_done": step, "generation": generation,
                               "final_loss": losses[-1] if losses else None, "rescales": rescales,
                               "recoveries": recoveries, "trace": trace}
+    if hasattr(adapter, "data_position"):
+        result["data_position"] = adapter.data_position
     if breaker is not None:
         breaker.stop()
     if _CKPT.get("writer") is not None:
@@ -725,7 +751,25 @@ def parse_args(argv=None):
     ap.add_argument("--ckpt-dir", default="")
     ap.add_argument("--ckpt-every", type=int, default=0)
     ap.add_argument("--step-sleep", type=float, default=0.0)
-    return ap.parse_args(argv)
+    ap.add_argument("--data", default="", metavar="PATH_OR_GLOB",
+                    help="train on these token shards (llm.c .bin shards or raw uint16 files; GPT-2 models) instead of "
+                         "synthetic tokens")
+    ap.add_argument("--doc-mask", action="store_true",
+                    help="with --data: a token attends only to earlier tokens of its own document (documents start at "
+                         "the end-of-text token); runs the wgmma attention kernels")
+    ap.add_argument("--eot-token", type=int, default=50256, help="end-of-text token id that starts a document")
+    args = ap.parse_args(argv)
+    if args.doc_mask and not args.data:
+        ap.error("--doc-mask needs --data")
+    if args.data and args.model not in ("gpt2", "gpt2-tiny"):
+        ap.error(f"--data trains GPT-2 models only, not {args.model}")
+    if args.data:
+        from ..models.gpt2 import GPT2Config
+
+        vocab = (GPT2Config.small() if args.model == "gpt2" else GPT2Config.tiny()).vocab_size
+        if args.doc_mask and not 0 <= args.eot_token < vocab:
+            ap.error(f"--eot-token {args.eot_token} is outside the vocabulary of {args.model} (size {vocab})")
+    return args
 
 
 def main(argv=None) -> int:
