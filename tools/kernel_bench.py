@@ -145,14 +145,16 @@ def main():
                  "gbs": byts / med / 1e6, "frac_of_measured_peak": frac(byts / med / 1e6, PEAK_BW)})
     med, best = timeit(lambda: F.sumsq(gr, ss))
     rows.append({"kernel": "sumsq", "ms_med": med, "ms_best": best, "gbs": n * 4 / med / 1e6,
-                 "frac_of_measured_peak": n * 4 / med / 1e6 / PEAK_BW})
+                 "frac_of_measured_peak": frac(n * 4 / med / 1e6, PEAK_BW)})
 
     os.makedirs("gpurun_out", exist_ok=True)
     json.dump({"peaks": {"bf16_tflops": PEAK_TF, "hbm_gbs": PEAK_BW}, "rows": rows},
               open("gpurun_out/kernel_bench.json", "w"), indent=1)
     for r in rows:
         perf = f"{r['tflops']:8.1f} TF" if "tflops" in r else f"{r['gbs']:8.1f} GB/s"
-        print(f"{r['kernel']:<52s} {r['ms_med']:8.3f} ms  {perf}  {100 * r['frac_of_measured_peak']:5.1f}% of measured")
+        share = r["frac_of_measured_peak"]
+        print(f"{r['kernel']:<52s} {r['ms_med']:8.3f} ms  {perf}  "
+              + (f"{100 * share:5.1f}% of measured" if share is not None else "(no measured peak)"))
 
 
 if __name__ == "__main__":

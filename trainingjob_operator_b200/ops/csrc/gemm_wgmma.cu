@@ -250,18 +250,15 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
     // ------------------------------------------------------------ consumers (warpgroups 1, 2: 64 rows each)
     asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n" ::: "memory");
     const int wg = (warp >> 2) - 1;
-    const bool signaller = (threadIdx.x & 127) == 0;
+    // lane c of the warpgroup's first warp frees the stage in CTA c of the cluster
+    const bool signaller = (threadIdx.x & 127) < kCM;
     float acc[kBN / 2];
     int stage = 0;
     uint32_t phase = 0;
     auto release = [&](int s) {
       if (signaller) {
-        if constexpr (kCM > 1) {
-#pragma unroll
-          for (int c = 0; c < kCM; ++c) mbar_arrive_remote(&empty_bar[s], static_cast<uint32_t>(c));
-        } else {
-          mbar_arrive(&empty_bar[s]);
-        }
+        if constexpr (kCM > 1) mbar_arrive_remote(&empty_bar[s], static_cast<uint32_t>(lane));
+        else mbar_arrive(&empty_bar[s]);
       }
     };
     for (int w = cluster_id; w < num_work; w += num_clusters) {

@@ -140,9 +140,12 @@ __device__ __forceinline__ uint32_t mapa_u32(uint32_t local_smem_addr, uint32_t 
   asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(local_smem_addr), "r"(cta));
   return r;
 }
+// Arrive on the mbarrier at the same offset as `bar` in CTA `cta` of this cluster, with the default .release.cta
+// semantics.  Enough to hand a ring stage back to a peer's producer after wgmma.wait_group has retired this thread's
+// reads of it; a .release.cluster arrive compiles to a GPU-scope MEMBAR on sm_90a, which stalls the whole warpgroup.
 __device__ __forceinline__ void mbar_arrive_remote(uint64_t* bar, uint32_t cta) {
   const uint32_t ra = mapa_u32(smem_u32(bar), cta);
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(ra) : "memory");
+  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(ra) : "memory");
 }
 __device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity) {
   const uint32_t addr = smem_u32(bar);

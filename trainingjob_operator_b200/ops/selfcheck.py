@@ -786,7 +786,69 @@ def case_gpt2_docs():
     return ok
 
 
+def case_gemm_cluster():
+    """Cluster kernels (block_n=512 / 1024), whose consumers hand each ring stage back to every CTA of the cluster: a
+    single work item, work items spread unevenly over the clusters, split-K whose last split is shorter, M, N and K tails, and
+    every epilogue flag a single GPU can run, the owner-sharded weight gradient included."""
+    import ctypes
+
+    ok = True
+    for bn in (512, 1024):
+        for (M, N, K, a_mn, b_mn, kw) in [(256, 128, 64, False, False, {}),             # one work item
+                                          (200, 136, 72, True, True, {}),               # one item, M / N / K tails
+                                          (512, 896, 320, False, False, {"max_ctas": 12}),  # 1 or 2 items per cluster
+                                          (1000, 904, 264, False, True, {"max_ctas": 8}),
+                                          (776, 520, 200, True, False, {"max_ctas": 4})]:
+            ok &= _gemm_case(M, N, K, a_mn, b_mn, block_n=bn, **kw)
+        M, N, K = 1000, 904, 1000          # 16 k-blocks in splits of 6, 6 and 4
+        a, b = _rand(M, K), _rand(N, K, scale=0.05)
+        bias, res = _rand(N), _rand(M, N)
+        pre_ref = a.float() @ b.float().t() + bias.float()
+        out = torch.empty(M, N, device="cuda", dtype=torch.bfloat16)
+        aux = torch.empty_like(out)
+        F.gemm(a, b, out, bias=bias, gelu=True, save_pre=True, aux=aux, block_n=bn, max_ctas=10)
+        ok &= _check(f"bn={bn} bias+gelu", out, torch.nn.functional.gelu(pre_ref, approximate="tanh"), 1e-2)
+        ok &= _check(f"bn={bn} save_pre", aux, pre_ref, 1e-2)
+        F.gemm(a, b, out, bias=bias, residual=res, block_n=bn)
+        ok &= _check(f"bn={bn} bias+residual", out, pre_ref + res.float(), 1e-2)
+        h = _rand(M, N)
+        hf = h.float().requires_grad_(True)
+        (gp,) = torch.autograd.grad(torch.nn.functional.gelu(hf, approximate="tanh").sum(), hf)
+        cs = torch.full((N,), 2.0, device="cuda")
+        F.gemm(a, b, out, dgelu=True, aux=h, block_n=bn, colsum=cs)
+        dy = a.float() @ b.float().t()
+        ok &= _check(f"bn={bn} dgelu", out, dy * gp, 2e-2)
+        ok &= _check(f"bn={bn} fused colsum", cs, out.float().sum(0) + 2.0, 1e-3)
+        o32 = torch.zeros(M, N, device="cuda", dtype=torch.float32)
+        F.gemm(a, b, o32, block_n=bn)
+        ok &= _check(f"bn={bn} out_f32", o32, dy, 1e-2)
+        o32.fill_(1.0)
+        F.gemm(a, b, o32, accumulate=True, split_k=3, block_n=bn, max_ctas=2 * (bn // 256))
+        ok &= _check(f"bn={bn} accumulate split_k=3 (6+6+4 k-blocks)", o32, dy + 1.0, 1e-2)
+        # owner-sharded weight gradient with an emulated second rank, with and without split-K (peer_move_kernel)
+        Mtok, Nout, Kin = 2048, 768, 1024
+        dyv, x = _rand(Mtok, Nout), _rand(Mtok, Kin)
+        ref = dyv.float().t() @ x.float()
+        half = Nout // 2
+        for sk_peer in (1, 3):
+            local = torch.zeros(Nout * Kin, device="cuda")
+            owner1 = torch.zeros(Nout * Kin, device="cuda")
+            delta = (ctypes.c_longlong * 8)(0, owner1.data_ptr() - local.data_ptr(), *([0] * 6))
+            bound = (ctypes.c_longlong * 9)(0, half * Kin, *([Nout * Kin] * 7))
+            assert F.lib.load().aitj_gemm_set_peers(ctypes.c_void_p(local.data_ptr()), delta, bound, 2) == 0
+            F.gemm(dyv, x, F.PeerView(local.view(Nout, Kin)), a_mn=True, b_mn=True, accumulate=True, split_k=sk_peer,
+                   block_n=bn)
+            torch.cuda.synchronize()
+            lo, hi = local.view(Nout, Kin), owner1.view(Nout, Kin)
+            ok &= _check(f"bn={bn} peer wgrad split_k={sk_peer}: owned rows", lo[:half], ref[:half], 1e-2)
+            ok &= _check(f"bn={bn} peer wgrad split_k={sk_peer}: other rows", hi[half:], ref[half:], 1e-2)
+            ok &= bool((lo[half:] == 0).all()) and bool((hi[:half] == 0).all())
+    torch.cuda.synchronize()
+    return ok
+
+
 CASES = {
+    "gemm_cluster": case_gemm_cluster,
     "attention": case_attention,
     "attention_docs": case_attention_docs,
     "gpt2_docs": case_gpt2_docs,
