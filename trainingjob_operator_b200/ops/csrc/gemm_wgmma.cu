@@ -17,6 +17,11 @@
 // same B tile: each CTA loads 1/kCM of it and multicasts the slice to every CTA of the cluster, so each B byte is read
 // from L2 once per cluster instead of once per CTA.  A stage is free again only when the consumers of every CTA of the
 // cluster have released it (a peer's multicast writes into this CTA's ring).
+//
+// The epilogue variant is a template parameter (kEpi, EPI_* bits), so a kernel contains only the paths its variant
+// uses.  An epilogue that tests every flag at run time unrolls to ~20k instructions per 256-wide kernel, and the
+// consumer warps fetch that code again on every tile; with a plain-store epilogue the whole kernel is under 1k.  Only
+// the (layout, epilogue) pairs in kGemmKernels are compiled; aitj_gemm_bf16 returns -7 for any other.
 #include "ptx.cuh"
 #include <string.h>
 
@@ -36,6 +41,7 @@ enum : int {
   EPI_OUT_F32 = 32,   // out is fp32 (plain store)
   EPI_ACCUM = 64,     // out is fp32, red.global.add (split-K / grad accumulation)
   EPI_MC = 128,       // with EPI_ACCUM: `out` is an NVSwitch multicast address; reduce with multimem.red (GEMM + all-reduce in one kernel)
+  EPI_COLSUM = 256,   // bf16 out only: colsum[N] += column sums of the stored output (set by aitj_gemm_set_colsum)
   EPI_PEER = 16384    // with EPI_ACCUM: `out` lies in the symmetric, owner-sharded gradient buffer; every element is added into the
                       // copy of the rank that owns it (red.global.add over NVLink peer memory): weight-gradient GEMM +
                       // reduce-scatter in one kernel.  With split-K the splits add into the local copy and
@@ -49,12 +55,11 @@ struct GemmArgs {
   const __nv_bfloat16* bias;
   const __nv_bfloat16* residual;
   __nv_bfloat16* aux;
-  int flags;
   int split_k;
   int tiles_m, tiles_n;
   int k_blocks, k_per_split;
-  // optional (bf16 output): colsum[N] += column sums of the stored output, i.e. the bias gradient of the layer whose
-  // input gradient this GEMM produces
+  // EPI_COLSUM: colsum[N] += column sums of the stored output, i.e. the bias gradient of the layer whose input gradient
+  // this GEMM produces
   float* colsum;
 };
 
@@ -87,11 +92,11 @@ __device__ __forceinline__ void red_add_v2_f32(float* p, float a, float b) {
 
 // Epilogue of one consumer warpgroup: its 64 rows x kBN columns of accumulators in the wgmma fragment layout -- register
 // 4j + 2h + e holds row (r_base + 8h), column (c_base + 8j + e).
-template <int kBN>
+template <int kBN, int kEpi>
 __device__ __forceinline__ void epilogue(const GemmArgs& a, float (&acc)[kBN / 2], int r_base, int c_base) {
-  const int flags = a.flags;
+  constexpr int flags = kEpi;
   const int lane = threadIdx.x & 31;
-  if (flags & (EPI_OUT_F32 | EPI_ACCUM)) {
+  if constexpr (flags & (EPI_OUT_F32 | EPI_ACCUM)) {
     float* obase = reinterpret_cast<float*>(a.out);
 #pragma unroll
     for (int j = 0; j < kBN / 8; ++j) {
@@ -103,9 +108,9 @@ __device__ __forceinline__ void epilogue(const GemmArgs& a, float (&acc)[kBN / 2
         if (row >= a.M) continue;
         float* p = obase + static_cast<size_t>(row) * a.ldc + col;
         const float x0 = acc[4 * j + 2 * h], x1 = acc[4 * j + 2 * h + 1];
-        if (!(flags & EPI_ACCUM)) {
+        if constexpr (!(flags & EPI_ACCUM)) {
           *reinterpret_cast<float2*>(p) = make_float2(x0, x1);
-        } else if (flags & EPI_MC) {
+        } else if constexpr ((flags & EPI_MC) != 0) {
           mc_red_add_f32(p, x0);
           mc_red_add_f32(p + 1, x1);
         } else {
@@ -121,7 +126,7 @@ __device__ __forceinline__ void epilogue(const GemmArgs& a, float (&acc)[kBN / 2
     const int col = c_base + 8 * j;
     if (col >= a.N) break;       // N % 8 == 0: a column pair is either wholly inside or wholly outside
     float2 bv = make_float2(0.f, 0.f);
-    if (flags & EPI_BIAS) bv = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(a.bias + col));
+    if constexpr ((flags & EPI_BIAS) != 0) bv = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(a.bias + col));
     float cs0 = 0.f, cs1 = 0.f;
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
@@ -129,14 +134,14 @@ __device__ __forceinline__ void epilogue(const GemmArgs& a, float (&acc)[kBN / 2
       if (row >= a.M) continue;
       const size_t off = static_cast<size_t>(row) * a.ldc + col;
       float x0 = acc[4 * j + 2 * h] + bv.x, x1 = acc[4 * j + 2 * h + 1] + bv.y;
-      if (flags & EPI_SAVE_PRE) *reinterpret_cast<uint32_t*>(a.aux + off) = pack_bf16x2(x0, x1);
-      if (flags & EPI_GELU) { x0 = gelu_tanh(x0); x1 = gelu_tanh(x1); }
-      if (flags & EPI_DGELU) {
+      if constexpr ((flags & EPI_SAVE_PRE) != 0) *reinterpret_cast<uint32_t*>(a.aux + off) = pack_bf16x2(x0, x1);
+      if constexpr ((flags & EPI_GELU) != 0) { x0 = gelu_tanh(x0); x1 = gelu_tanh(x1); }
+      if constexpr ((flags & EPI_DGELU) != 0) {
         const float2 pre = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(a.aux + off));
         x0 *= gelu_tanh_grad(pre.x);
         x1 *= gelu_tanh_grad(pre.y);
       }
-      if (flags & EPI_RESIDUAL) {
+      if constexpr ((flags & EPI_RESIDUAL) != 0) {
         const float2 r = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(a.residual + off));
         x0 += r.x;
         x1 += r.y;
@@ -147,7 +152,7 @@ __device__ __forceinline__ void epilogue(const GemmArgs& a, float (&acc)[kBN / 2
       cs0 += stored.x;
       cs1 += stored.y;
     }
-    if (a.colsum != nullptr) {
+    if constexpr ((flags & EPI_COLSUM) != 0) {
       // the eight lanes with the same (lane & 3) hold the same two columns of the warp's 16 rows
 #pragma unroll
       for (int o = 4; o < 32; o <<= 1) {
@@ -167,7 +172,7 @@ __host__ __device__ constexpr int gemm_stages() { return kBN == 256 ? 4 : 6; }
 template <int kBN>
 __host__ __device__ constexpr int gemm_smem_bytes() { return gemm_stages<kBN>() * (BLOCK_M + kBN) * BLOCK_K * 2 + 1024 + 256; }
 
-template <int kBN, bool kAMN, bool kBMN, int kCM>
+template <int kBN, bool kAMN, bool kBMN, int kCM, int kEpi>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                        const GemmArgs args) {
@@ -291,7 +296,7 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
       if (nk > 0) {
         const int wl = warp & 3;
         const int m_blk = wi.m_blk * kCM + static_cast<int>(rank);
-        epilogue<kBN>(args, acc, m_blk * BLOCK_M + wg * 64 + wl * 16 + (lane >> 2), wi.n_blk * kBN + 2 * (lane & 3));
+        epilogue<kBN, kEpi>(args, acc, m_blk * BLOCK_M + wg * 64 + wl * 16 + (lane >> 2), wi.n_blk * kBN + 2 * (lane & 3));
       }
     }
   }
@@ -363,12 +368,12 @@ static int num_sms() {
   return n;
 }
 
-template <int kBN, bool kAMN, bool kBMN, int kCM>
+template <int kBN, bool kAMN, bool kBMN, int kCM, int kEpi>
 static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const GemmArgs& args, int max_ctas,
                        cudaStream_t stream) {
   constexpr int kSmem = gemm_smem_bytes<kBN>();
   static int max_clusters = 0;
-  auto kern = gemm_bf16_wgmma_kernel<kBN, kAMN, kBMN, kCM>;
+  auto kern = gemm_bf16_wgmma_kernel<kBN, kAMN, kBMN, kCM, kEpi>;
   cudaLaunchConfig_t cfg = {};
   cudaLaunchAttribute at[1];
   at[0].id = cudaLaunchAttributeClusterDimension;
@@ -400,6 +405,50 @@ static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const GemmA
   return cudaPeekAtLastError() == cudaSuccess ? 0 : -30;
 }
 
+typedef int (*LaunchFn)(const CUtensorMap&, const CUtensorMap&, const GemmArgs&, int, cudaStream_t);
+
+struct GemmKernel {
+  bool a_mn, b_mn;
+  int epi;            // EPI_* bits, EPI_COLSUM included
+  int block_n, cm;    // tile width and CTAs per cluster
+  LaunchFn launch;
+};
+
+// Every tile configuration of one (operand layout, epilogue) pair: 128- and 256-wide tiles on single CTAs, and 256-wide
+// tiles in clusters of 2 and 4.
+#define GEMM_TILES(AMN, BMN, EPI)                          \
+  {AMN, BMN, EPI, 128, 1, launch_gemm<128, AMN, BMN, 1, EPI>},  \
+  {AMN, BMN, EPI, 256, 1, launch_gemm<256, AMN, BMN, 1, EPI>},  \
+  {AMN, BMN, EPI, 256, 2, launch_gemm<256, AMN, BMN, 2, EPI>},  \
+  {AMN, BMN, EPI, 256, 4, launch_gemm<256, AMN, BMN, 4, EPI>}
+
+// The kernels aitj_gemm_bf16 can launch: the epilogues GPT2Engine and BertEngine use (BERT shares GPT-2's GEMM
+// front-ends) and the ones ops/selfcheck.py checks.
+static const GemmKernel kGemmKernels[] = {
+    // forward, x[M,K] @ W[N,K]^T: logits; qkv; fc (+ GELU, pre-activation saved); attn proj and fc2 (+ skip connection)
+    GEMM_TILES(false, false, 0),
+    GEMM_TILES(false, false, EPI_BIAS),
+    GEMM_TILES(false, false, EPI_BIAS | EPI_GELU | EPI_SAVE_PRE),
+    GEMM_TILES(false, false, EPI_BIAS | EPI_RESIDUAL),
+    // epilogues of the other layouts, checked on this one (selfcheck)
+    GEMM_TILES(false, false, EPI_DGELU),
+    GEMM_TILES(false, false, EPI_DGELU | EPI_COLSUM),
+    GEMM_TILES(false, false, EPI_OUT_F32),
+    GEMM_TILES(false, false, EPI_ACCUM),
+    // input gradient, dy[M,N] @ W[N,K]: fc2 (* GELU', + fc bias gradient); qkv with the skip connection's gradient (BERT)
+    GEMM_TILES(false, true, 0),
+    GEMM_TILES(false, true, EPI_DGELU),
+    GEMM_TILES(false, true, EPI_DGELU | EPI_COLSUM),
+    GEMM_TILES(false, true, EPI_RESIDUAL),
+    // weight gradient, dW[N,K] += dy[M,N]^T x[M,K]: local, NVSwitch multicast, owner-sharded
+    GEMM_TILES(true, true, 0),
+    GEMM_TILES(true, true, EPI_ACCUM),
+    GEMM_TILES(true, true, EPI_ACCUM | EPI_MC),
+    GEMM_TILES(true, true, EPI_ACCUM | EPI_PEER),
+    GEMM_TILES(true, false, 0),
+};
+#undef GEMM_TILES
+
 }  // namespace aitj
 
 static float* g_gemm_colsum = nullptr;   // consumed by the next aitj_gemm_bf16 call
@@ -412,7 +461,8 @@ int aitj_gemm_set_colsum(void* buf) { g_gemm_colsum = reinterpret_cast<float*>(b
 
 // Returns 0 on success. See file header for operand conventions. lda/ldb/ldc in elements.
 // block_n: 128 or 256 (0 = auto); 512 / 1024: 128x256 tiles in clusters of 2 / 4 CTAs sharing B by TMA multicast.
-// split_k > 1 requires EPI_ACCUM. max_ctas: 0 = all SMs.
+// split_k > 1 requires EPI_ACCUM. max_ctas: 0 = all SMs.  -7: no kernel is compiled for this operand layout and
+// epilogue (kGemmKernels).
 int aitj_gemm_bf16(const void* A, const void* B, void* out, int M, int N, int K, int lda, int ldb, int ldc,
                    int a_mn, int b_mn, const void* bias, const void* residual, void* aux, int flags, int split_k,
                    int block_n, int max_ctas, void* stream_ptr) {
@@ -433,7 +483,6 @@ int aitj_gemm_bf16(const void* A, const void* B, void* out, int M, int N, int K,
   args.bias = reinterpret_cast<const __nv_bfloat16*>(bias);
   args.residual = reinterpret_cast<const __nv_bfloat16*>(residual);
   args.aux = reinterpret_cast<__nv_bfloat16*>(aux);
-  args.flags = flags;
   args.colsum = g_gemm_colsum;
   g_gemm_colsum = nullptr;
   if (args.colsum && (flags & (EPI_OUT_F32 | EPI_ACCUM))) return -6;   // column sums of a bf16 output only
@@ -444,6 +493,14 @@ int aitj_gemm_bf16(const void* A, const void* B, void* out, int M, int N, int K,
   if (split_k > args.k_blocks) split_k = args.k_blocks;
   args.k_per_split = (args.k_blocks + split_k - 1) / split_k;
   args.split_k = (args.k_blocks + args.k_per_split - 1) / args.k_per_split;
+  const bool peer_move = (flags & EPI_PEER) && args.split_k > 1;
+  int epi = flags & ~EPI_COLSUM;
+  if (args.colsum) epi |= EPI_COLSUM;
+  if (peer_move) epi &= ~EPI_PEER;
+  const GemmKernel* kernel = nullptr;
+  for (const GemmKernel& k : kGemmKernels)
+    if (k.a_mn == (a_mn != 0) && k.b_mn == (b_mn != 0) && k.epi == epi && k.block_n == block_n && k.cm == cm) kernel = &k;
+  if (!kernel) return -7;
 
   CUtensorMap ta, tb;
   int rc;
@@ -453,19 +510,7 @@ int aitj_gemm_bf16(const void* A, const void* B, void* out, int M, int N, int K,
   if (!b_mn) rc = encode_2d(&tb, B, K, N, ldb, BLOCK_K, block_n / cm);
   else       rc = encode_2d(&tb, B, N, K, ldb, 64, BLOCK_K);
   if (rc) return rc - 1000;
-  const bool peer_move = (flags & EPI_PEER) && args.split_k > 1;
-  if (peer_move) args.flags &= ~EPI_PEER;
-
-#define AITJ_DISPATCH(BN, CM)                                                                         \
-  if (!a_mn && !b_mn) rc = launch_gemm<BN, false, false, CM>(ta, tb, args, max_ctas, stream);        \
-  else if (!a_mn && b_mn) rc = launch_gemm<BN, false, true, CM>(ta, tb, args, max_ctas, stream);     \
-  else if (a_mn && !b_mn) rc = launch_gemm<BN, true, false, CM>(ta, tb, args, max_ctas, stream);     \
-  else rc = launch_gemm<BN, true, true, CM>(ta, tb, args, max_ctas, stream);
-  if (cm == 4) { AITJ_DISPATCH(256, 4) }
-  else if (cm == 2) { AITJ_DISPATCH(256, 2) }
-  else if (block_n == 256) { AITJ_DISPATCH(256, 1) }
-  else { AITJ_DISPATCH(128, 1) }
-#undef AITJ_DISPATCH
+  rc = kernel->launch(ta, tb, args, max_ctas, stream);
   if (rc || !peer_move) return rc;
   const size_t nvec = static_cast<size_t>(M) * (N / 4);
   int blocks = static_cast<int>((nvec + 255) / 256);

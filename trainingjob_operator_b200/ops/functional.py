@@ -19,6 +19,10 @@ EPI_OUT_F32 = 32
 EPI_ACCUM = 64
 EPI_MC = 128
 EPI_PEER = 16384
+EPI_COLSUM = 256   # set by the library when a colsum buffer is given
+
+# aitj_gemm_bf16: no kernel is compiled for this operand layout and epilogue
+GEMM_NO_KERNEL = -7
 
 
 class RawView:
@@ -112,6 +116,34 @@ def gemm(a, b, out, *, a_mn=False, b_mn=False, bias=None, residual=None, aux=Non
         N, Kb = b.shape
     assert K == Kb, (a.shape, b.shape, a_mn, b_mn)
     assert out.shape[0] == M and out.shape[1] == N, (out.shape, M, N)
+    flags = gemm_epilogue(out, bias=bias, residual=residual, aux=aux, gelu=gelu, dgelu=dgelu, save_pre=save_pre,
+                          accumulate=accumulate, colsum=colsum)
+    if colsum is not None:
+        lib.load().aitj_gemm_set_colsum(colsum.data_ptr())
+    try:
+        lib.call("aitj_gemm_bf16", a.data_ptr(), b.data_ptr(), out.data_ptr(), M, N, K, a.stride(0), b.stride(0),
+                 out.stride(0), int(a_mn), int(b_mn), _ptr(bias), _ptr(residual), _ptr(aux), flags & ~EPI_COLSUM,
+                 int(split_k), int(block_n), int(max_ctas), _stream())
+    except lib.KernelError as e:
+        if e.code != GEMM_NO_KERNEL:
+            raise
+        raise lib.KernelError(f"no wgmma GEMM kernel is compiled for a_mn={int(a_mn)} b_mn={int(b_mn)} with epilogue "
+                              f"{epilogue_name(flags)}; add the pair to kGemmKernels in gemm_wgmma.cu",
+                              e.code) from None
+    return out
+
+
+def epilogue_name(flags: int) -> str:
+    names = [n for n, bit in (("BIAS", EPI_BIAS), ("GELU", EPI_GELU), ("RESIDUAL", EPI_RESIDUAL),
+                              ("SAVE_PRE", EPI_SAVE_PRE), ("DGELU", EPI_DGELU), ("OUT_F32", EPI_OUT_F32),
+                              ("ACCUM", EPI_ACCUM), ("MC", EPI_MC), ("PEER", EPI_PEER), ("COLSUM", EPI_COLSUM))
+             if flags & bit]
+    return "|".join(names) or "none"
+
+
+def gemm_epilogue(out, *, bias=None, residual=None, aux=None, gelu=False, dgelu=False, save_pre=False,
+                  accumulate=False, colsum=None) -> int:
+    """The EPI_* bits of a ``gemm`` call with these arguments; EPI_COLSUM marks a colsum buffer."""
     flags = 0
     if bias is not None:
         flags |= EPI_BIAS
@@ -137,12 +169,9 @@ def gemm(a, b, out, *, a_mn=False, b_mn=False, bias=None, residual=None, aux=Non
     else:
         assert out.dtype == torch.bfloat16 and not accumulate
     if colsum is not None:
-        assert colsum.dtype == torch.float32 and colsum.numel() == N and out.dtype == torch.bfloat16
-        lib.load().aitj_gemm_set_colsum(colsum.data_ptr())
-    lib.call("aitj_gemm_bf16", a.data_ptr(), b.data_ptr(), out.data_ptr(), M, N, K, a.stride(0), b.stride(0),
-             out.stride(0), int(a_mn), int(b_mn), _ptr(bias), _ptr(residual), _ptr(aux), flags, int(split_k),
-             int(block_n), int(max_ctas), _stream())
-    return out
+        assert colsum.dtype == torch.float32 and colsum.numel() == out.shape[1] and out.dtype == torch.bfloat16
+        flags |= EPI_COLSUM
+    return flags
 
 
 def auto_split_k(M: int, N: int, K: int, block_n: int = 0, pair: bool = False) -> int:

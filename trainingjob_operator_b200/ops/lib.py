@@ -23,7 +23,9 @@ LAUNCHES = 0
 
 
 class KernelError(RuntimeError):
-    pass
+    def __init__(self, msg: str, code: int = 0):
+        super().__init__(msg)
+        self.code = code
 
 
 def load(build_if_missing: bool = True):
@@ -155,6 +157,6 @@ def call(name: str, *args) -> int:
     else:
         rc = getattr(lib, name)(*args)
     if rc != 0:
-        raise KernelError(f"{name} failed with code {rc}")
+        raise KernelError(f"{name} failed with code {rc}", rc)
     LAUNCHES += 1
     return rc
