@@ -1,6 +1,7 @@
 // Persistent, warp-specialised bf16 GEMM for sm_90a (H100): TMA -> 128B-swizzled shared-memory ring -> wgmma with the
-// fp32 accumulators in registers -> epilogue straight from the registers with fused bias / GELU / dGELU / residual /
-// pre-activation save, fp32 store or fp32 reduce-add (split-K, gradient accumulation) and optional column sums.
+// fp32 accumulators in registers -> epilogue with fused bias / GELU / dGELU / residual / pre-activation save and
+// optional column sums, whose bf16 outputs leave through shared memory by TMA store (inputs arrive by TMA load), or an
+// fp32 store or fp32 reduce-add (split-K, gradient accumulation) straight from the registers.
 //
 //   out[M,N] (+)= opA[M,K] * opB[N,K]^T
 //     a_mn == 0 : A stored [M,K] row-major (K contiguous, "K-major")
@@ -90,104 +91,205 @@ __device__ __forceinline__ void red_add_v2_f32(float* p, float a, float b) {
   asm volatile("red.global.add.v2.f32 [%0], {%1,%2};" ::"l"(p), "f"(a), "f"(b) : "memory");
 }
 
-// Epilogue of one consumer warpgroup: its 64 rows x kBN columns of accumulators in the wgmma fragment layout -- register
-// 4j + 2h + e holds row (r_base + 8h), column (c_base + 8j + e).
+template <int kEpi>
+__host__ __device__ constexpr bool bf16_out() { return (kEpi & (EPI_OUT_F32 | EPI_ACCUM)) == 0; }
+// bf16 epilogues that read a second [M, ldc] input: the residual, or the saved pre-activation for GELU'
+template <int kEpi>
+__host__ __device__ constexpr bool epi_reads() { return (kEpi & (EPI_RESIDUAL | EPI_DGELU)) != 0; }
+
+// fp32 epilogue of one consumer warpgroup: its 64 rows x kBN columns of accumulators in the wgmma fragment layout --
+// register 4j + 2h + e holds row (r_base + 8h), column (c_base + 8j + e).
 template <int kBN, int kEpi>
-__device__ __forceinline__ void epilogue(const GemmArgs& a, float (&acc)[kBN / 2], int r_base, int c_base) {
+__device__ __forceinline__ void epilogue_f32(const GemmArgs& a, float (&acc)[kBN / 2], int r_base, int c_base) {
   constexpr int flags = kEpi;
-  const int lane = threadIdx.x & 31;
-  if constexpr (flags & (EPI_OUT_F32 | EPI_ACCUM)) {
-    float* obase = reinterpret_cast<float*>(a.out);
-#pragma unroll
-    for (int j = 0; j < kBN / 8; ++j) {
-      const int col = c_base + 8 * j;
-      if (col >= a.N) break;
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int row = r_base + 8 * h;
-        if (row >= a.M) continue;
-        float* p = obase + static_cast<size_t>(row) * a.ldc + col;
-        const float x0 = acc[4 * j + 2 * h], x1 = acc[4 * j + 2 * h + 1];
-        if constexpr (!(flags & EPI_ACCUM)) {
-          *reinterpret_cast<float2*>(p) = make_float2(x0, x1);
-        } else if constexpr ((flags & EPI_MC) != 0) {
-          mc_red_add_f32(p, x0);
-          mc_red_add_f32(p + 1, x1);
-        } else {
-          red_add_v2_f32((flags & EPI_PEER) ? peer_ptr(p) : p, x0, x1);
-        }
-      }
-    }
-    return;
-  }
-  __nv_bfloat16* out = reinterpret_cast<__nv_bfloat16*>(a.out);
+  float* obase = reinterpret_cast<float*>(a.out);
 #pragma unroll
   for (int j = 0; j < kBN / 8; ++j) {
     const int col = c_base + 8 * j;
-    if (col >= a.N) break;       // N % 8 == 0: a column pair is either wholly inside or wholly outside
-    float2 bv = make_float2(0.f, 0.f);
-    if constexpr ((flags & EPI_BIAS) != 0) bv = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(a.bias + col));
-    float cs0 = 0.f, cs1 = 0.f;
+    if (col >= a.N) break;
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const int row = r_base + 8 * h;
       if (row >= a.M) continue;
-      const size_t off = static_cast<size_t>(row) * a.ldc + col;
-      float x0 = acc[4 * j + 2 * h] + bv.x, x1 = acc[4 * j + 2 * h + 1] + bv.y;
-      if constexpr ((flags & EPI_SAVE_PRE) != 0) *reinterpret_cast<uint32_t*>(a.aux + off) = pack_bf16x2(x0, x1);
-      if constexpr ((flags & EPI_GELU) != 0) { x0 = gelu_tanh(x0); x1 = gelu_tanh(x1); }
-      if constexpr ((flags & EPI_DGELU) != 0) {
-        const float2 pre = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(a.aux + off));
-        x0 *= gelu_tanh_grad(pre.x);
-        x1 *= gelu_tanh_grad(pre.y);
-      }
-      if constexpr ((flags & EPI_RESIDUAL) != 0) {
-        const float2 r = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(a.residual + off));
-        x0 += r.x;
-        x1 += r.y;
-      }
-      const uint32_t packed = pack_bf16x2(x0, x1);
-      *reinterpret_cast<uint32_t*>(out + off) = packed;
-      const float2 stored = unpack_bf16x2(packed);
-      cs0 += stored.x;
-      cs1 += stored.y;
-    }
-    if constexpr ((flags & EPI_COLSUM) != 0) {
-      // the eight lanes with the same (lane & 3) hold the same two columns of the warp's 16 rows
-#pragma unroll
-      for (int o = 4; o < 32; o <<= 1) {
-        cs0 += __shfl_xor_sync(0xffffffffu, cs0, o);
-        cs1 += __shfl_xor_sync(0xffffffffu, cs1, o);
-      }
-      if (lane < 4) {
-        atomicAdd(a.colsum + col, cs0);
-        atomicAdd(a.colsum + col + 1, cs1);
+      float* p = obase + static_cast<size_t>(row) * a.ldc + col;
+      const float x0 = acc[4 * j + 2 * h], x1 = acc[4 * j + 2 * h + 1];
+      if constexpr (!(flags & EPI_ACCUM)) {
+        *reinterpret_cast<float2*>(p) = make_float2(x0, x1);
+      } else if constexpr ((flags & EPI_MC) != 0) {
+        mc_red_add_f32(p, x0);
+        mc_red_add_f32(p + 1, x1);
+      } else {
+        red_add_v2_f32((flags & EPI_PEER) ? peer_ptr(p) : p, x0, x1);
       }
     }
   }
 }
 
+// bf16 epilogues leave through shared memory.  Each consumer warpgroup owns two 8 KB slots; a slot holds one 64 x 64
+// box of a bf16 tensor map with SWIZZLE_128B (row r at byte 128 r, its 16-byte chunk c at chunk c ^ (r % 8)), so the
+// stmatrix / ldmatrix rows of one 8 x 8 matrix fall on eight different chunks and never share a bank.  The warpgroup
+// stages its 64 x kBN share one box ("unit") at a time, alternating slots, and one thread stores each box with TMA:
+// whole 128-byte lines leave in the background instead of 8-row x 16-byte scattered stores, and the tensor map's
+// bounds clip the M and N tails.  The warpgroup never waits for a store's writes, only (before it reuses a slot) for
+// the store to have read the slot.  RESIDUAL and DGELU inputs arrive by TMA in the slot their output leaves from.
+constexpr int kSlotBytes = 64 * 64 * 2;
+constexpr int kStagingBytes = 2 * 2 * kSlotBytes;   // 2 consumer warpgroups x 2 slots
+
+struct Staging {
+  uint8_t* slots;      // this warpgroup's two slots
+  uint64_t* in_bar;    // [2]: a slot's input box has landed (RESIDUAL / DGELU)
+  uint32_t unit;       // boxes staged so far; box u goes through slot u % 2
+  uint32_t in_phase;   // parity of each in_bar
+  int wg;
+  bool issuer;         // thread 0 of the warpgroup issues its TMA loads and stores
+};
+
+// Shared address of the 16-byte row of fragment group p (columns 16p .. 16p + 15 of a box) that this lane gives to
+// stmatrix / ldmatrix: lanes 8i .. 8i + 7 address the rows of matrix i = (8-column half i / 2, 8-row half i % 2).
+__device__ __forceinline__ uint32_t box_addr(const uint8_t* slot, int p) {
+  const int lane = threadIdx.x & 31;
+  const int row = ((threadIdx.x >> 5) & 3) * 16 + (lane & 8) + (lane & 7);
+  return smem_u32(slot) + row * 128 + (((2 * p + (lane >> 4)) ^ (lane & 7)) << 4);
+}
+
+// Load the input box at column c0, row m0 into slot s, the slot its output will leave from.
+__device__ __forceinline__ void load_input_box(Staging& st, const CUtensorMap* in_map, uint32_t s, int c0, int m0) {
+  mbar_arrive_expect_tx(&st.in_bar[s], kSlotBytes);
+  tma_load_2d(st.slots + s * kSlotBytes, in_map, &st.in_bar[s], c0, m0);
+}
+
+// Stage box `cb` (columns n0 + 64 cb ..) of the warpgroup's share in the next slot and store it through `map`: the
+// pre-activation if kPre, else the epilogue's output, computed exactly as a register epilogue would, in the same order.
+// The box is written in four 16-column groups, one stmatrix each, so that only four packed registers are live beside
+// the accumulators.
+template <int kBN, int kEpi, bool kPre>
+__device__ __forceinline__ void stage_box(const GemmArgs& a, const CUtensorMap* map, const CUtensorMap* in_map,
+                                          float (&acc)[kBN / 2], Staging& st, int cb, int m0, int n0) {
+  constexpr int flags = kEpi;
+  constexpr bool kReads = epi_reads<kEpi>() && !kPre;
+  const int lane = threadIdx.x & 31;
+  const int row = m0 + ((threadIdx.x >> 5) & 3) * 16 + (lane >> 2);   // rows row and row + 8 of the fragments
+  const uint32_t s = st.unit & 1u;
+  uint8_t* slot = st.slots + s * kSlotBytes;
+  if constexpr (kReads) {
+    mbar_wait(&st.in_bar[s], (st.in_phase >> s) & 1u);
+    st.in_phase ^= 1u << s;
+  }
+#pragma unroll
+  for (int p = 0; p < 4; ++p) {
+    uint32_t v[4];   // matrix i of the group: pair (j = 8 cb + 2p + i / 2, h = i % 2) of the register layout
+    if constexpr (kReads) ldmatrix_x4(box_addr(slot, p), v);
+#pragma unroll
+    for (int q = 0; q < 2; ++q) {
+      const int j = 8 * cb + 2 * p + q;
+      const int col = n0 + 8 * j + 2 * (lane & 3);
+      float2 bv = make_float2(0.f, 0.f);
+      if constexpr ((flags & EPI_BIAS) != 0)
+        if (col < a.N) bv = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(a.bias + col));
+      float cs0 = 0.f, cs1 = 0.f;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        float x0 = acc[4 * j + 2 * h] + bv.x, x1 = acc[4 * j + 2 * h + 1] + bv.y;
+        if constexpr (kPre) {
+          v[2 * q + h] = pack_bf16x2(x0, x1);
+          continue;
+        }
+        if constexpr ((flags & EPI_GELU) != 0) { x0 = gelu_tanh(x0); x1 = gelu_tanh(x1); }
+        if constexpr ((flags & EPI_DGELU) != 0) {
+          const float2 pre = unpack_bf16x2(v[2 * q + h]);
+          x0 *= gelu_tanh_grad(pre.x);
+          x1 *= gelu_tanh_grad(pre.y);
+        }
+        if constexpr ((flags & EPI_RESIDUAL) != 0) {
+          const float2 r = unpack_bf16x2(v[2 * q + h]);
+          x0 += r.x;
+          x1 += r.y;
+        }
+        const uint32_t packed = pack_bf16x2(x0, x1);
+        v[2 * q + h] = packed;
+        if constexpr ((flags & EPI_COLSUM) != 0) {
+          if (row + 8 * h < a.M) {
+            const float2 stored = unpack_bf16x2(packed);
+            cs0 += stored.x;
+            cs1 += stored.y;
+          }
+        }
+      }
+      if constexpr (!kPre && (flags & EPI_COLSUM) != 0) {
+        // the eight lanes with the same (lane & 3) hold the same two columns of the warp's 16 rows
+#pragma unroll
+        for (int o = 4; o < 32; o <<= 1) {
+          cs0 += __shfl_xor_sync(0xffffffffu, cs0, o);
+          cs1 += __shfl_xor_sync(0xffffffffu, cs1, o);
+        }
+        if (lane < 4 && col < a.N) {
+          atomicAdd(a.colsum + col, cs0);
+          atomicAdd(a.colsum + col + 1, cs1);
+        }
+      }
+    }
+    stmatrix_x4(box_addr(slot, p), v[0], v[1], v[2], v[3]);
+  }
+  fence_proxy_async_smem();
+  // the previous box's store has read the other slot: once the barrier is passed, the next box may be written there
+  if (st.issuer) tma_store_wait_read<0>();
+  named_bar_sync(1 + st.wg, 128);
+  if (st.issuer) {
+    tma_store_2d(map, slot, n0 + 64 * cb, m0);
+    tma_store_commit();
+    // this slot receives the input of the box after next once the store has read it
+    if (kReads && cb + 2 < kBN / 64 && n0 + 64 * (cb + 2) < a.N) {
+      tma_store_wait_read<0>();
+      load_input_box(st, in_map, s, n0 + 64 * (cb + 2), m0);
+    }
+  }
+  ++st.unit;
+}
+
+// bf16 epilogue of one consumer warpgroup: rows m0 .. m0 + 63, columns n0 .. n0 + kBN - 1, accumulators in the
+// register layout of epilogue_f32.
+template <int kBN, int kEpi>
+__device__ __forceinline__ void epilogue_bf16(const GemmArgs& a, const CUtensorMap* out_map, const CUtensorMap* aux_map,
+                                              const CUtensorMap* in_map, float (&acc)[kBN / 2], Staging& st, int m0,
+                                              int n0) {
+#pragma unroll
+  for (int cb = 0; cb < kBN / 64; ++cb) {
+    if (n0 + 64 * cb >= a.N) break;
+    if constexpr ((kEpi & EPI_SAVE_PRE) != 0) stage_box<kBN, kEpi, true>(a, aux_map, in_map, acc, st, cb, m0, n0);
+    stage_box<kBN, kEpi, false>(a, out_map, in_map, acc, st, cb, m0, n0);
+  }
+}
+
 template <int kBN>
 __host__ __device__ constexpr int gemm_stages() { return kBN == 256 ? 4 : 6; }
-template <int kBN>
-__host__ __device__ constexpr int gemm_smem_bytes() { return gemm_stages<kBN>() * (BLOCK_M + kBN) * BLOCK_K * 2 + 1024 + 256; }
+template <int kBN, int kEpi>
+__host__ __device__ constexpr int gemm_smem_bytes() {
+  return gemm_stages<kBN>() * (BLOCK_M + kBN) * BLOCK_K * 2 + (bf16_out<kEpi>() ? kStagingBytes : 0) + 1024 + 256;
+}
 
 template <int kBN, bool kAMN, bool kBMN, int kCM, int kEpi>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-                       const GemmArgs args) {
+                       const __grid_constant__ CUtensorMap tmap_out, const __grid_constant__ CUtensorMap tmap_aux,
+                       const __grid_constant__ CUtensorMap tmap_res, const GemmArgs args) {
   constexpr int kStages = gemm_stages<kBN>();
   constexpr int kStageA = BLOCK_M * BLOCK_K * 2;
   constexpr int kStageB = kBN * BLOCK_K * 2;
   constexpr int kStageBytes = kStageA + kStageB;
   constexpr int kSliceN = kBN / kCM;               // rows of the B tile this CTA loads and multicasts
   static_assert(!kBMN || kSliceN % 64 == 0, "MN-major B slices are whole 64-column chunks");
+  static_assert(!(kEpi & EPI_RESIDUAL) || !(kEpi & (EPI_DGELU | EPI_SAVE_PRE)), "one second bf16 tensor per epilogue");
+  static_assert(!(kEpi & EPI_DGELU) || !(kEpi & EPI_SAVE_PRE), "one second bf16 tensor per epilogue");
+  constexpr int kStaging = bf16_out<kEpi>() ? kStagingBytes : 0;
+  const CUtensorMap* in_map = (kEpi & EPI_RESIDUAL) ? &tmap_res : &tmap_aux;
 
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_addr = smem_u32(smem_raw);
   uint8_t* smem = smem_raw + ((1024u - (raw_addr & 1023u)) & 1023u);
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kStages * kStageBytes);
+  uint8_t* staging = smem + kStages * kStageBytes;   // 1024-aligned: every stage is a multiple of 1024 bytes
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(staging + kStaging);
   uint64_t* empty_bar = full_bar + kStages;
+  uint64_t* in_bar = empty_bar + kStages;             // [2 warpgroups][2 slots]
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -196,10 +298,15 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmap_a);
     tma_prefetch_desc(&tmap_b);
+    if constexpr (bf16_out<kEpi>()) tma_prefetch_desc(&tmap_out);
+    if constexpr ((kEpi & EPI_SAVE_PRE) != 0) tma_prefetch_desc(&tmap_aux);
+    if constexpr (epi_reads<kEpi>()) tma_prefetch_desc(in_map);
     for (int i = 0; i < kStages; ++i) {
       mbar_init(&full_bar[i], 1);          // this CTA's producer: arrive(expect_tx) + the bytes of A and all B slices
       mbar_init(&empty_bar[i], 2 * kCM);   // both consumer warpgroups of every CTA of the cluster
     }
+    if constexpr (epi_reads<kEpi>())
+      for (int i = 0; i < 4; ++i) mbar_init(&in_bar[i], 1);   // the warpgroup's issuer: arrive(expect_tx) + one box
     fence_barrier_init();
   }
   if constexpr (kCM > 1) cluster_sync_all();   // no multicast may reach a peer before its barriers exist
@@ -260,6 +367,7 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
     float acc[kBN / 2];
     int stage = 0;
     uint32_t phase = 0;
+    Staging st{staging + wg * 2 * kSlotBytes, in_bar + 2 * wg, 0u, 0u, wg, (threadIdx.x & 127) == 0};
     auto release = [&](int s) {
       if (signaller) {
         if constexpr (kCM > 1) mbar_arrive_remote(&empty_bar[s], static_cast<uint32_t>(lane));
@@ -269,6 +377,8 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
     for (int w = cluster_id; w < num_work; w += num_clusters) {
       const WorkItem wi = decode_work(sched, w);
       const int nk = wi.kb1 - wi.kb0;
+      const int m0 = (wi.m_blk * kCM + static_cast<int>(rank)) * BLOCK_M + wg * 64;   // this warpgroup's rows
+      const int n0 = wi.n_blk * kBN;
       int prev = -1;
       for (int kb = 0; kb < nk; ++kb) {
         mbar_wait(&full_bar[stage], phase);
@@ -285,6 +395,16 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
           else wgmma_m64n128_ss<kAMN, kBMN>(acc, da, db, (kb > 0 || ks > 0) ? 1 : 0);
         }
         wgmma_commit();
+        if constexpr (epi_reads<kEpi>()) {
+          // the epilogue's first two input boxes load under the first k-block's MMAs, as soon as the previous tile's
+          // last stores have read their slots
+          if (kb == 0 && st.issuer && m0 < args.M) {
+            tma_store_wait_read<0>();
+#pragma unroll
+            for (int cb = 0; cb < 2; ++cb)
+              if (n0 + 64 * cb < args.N) load_input_box(st, in_map, (st.unit + cb) & 1u, n0 + 64 * cb, m0);
+          }
+        }
         wgmma_wait<1>();            // the previous stage's MMAs have retired: its buffers can be refilled
         if (prev >= 0) release(prev);
         prev = stage;
@@ -294,11 +414,16 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
       fence_regs(acc);
       if (prev >= 0) release(prev);
       if (nk > 0) {
-        const int wl = warp & 3;
-        const int m_blk = wi.m_blk * kCM + static_cast<int>(rank);
-        epilogue<kBN, kEpi>(args, acc, m_blk * BLOCK_M + wg * 64 + wl * 16 + (lane >> 2), wi.n_blk * kBN + 2 * (lane & 3));
+        if constexpr (bf16_out<kEpi>()) {
+          if (m0 < args.M) epilogue_bf16<kBN, kEpi>(args, &tmap_out, &tmap_aux, in_map, acc, st, m0, n0);
+        } else {
+          epilogue_f32<kBN, kEpi>(args, acc, m0 + (warp & 3) * 16 + (lane >> 2), n0 + 2 * (lane & 3));
+        }
       }
     }
+    // the shared memory of the last stores stays valid until they have read it
+    if constexpr (bf16_out<kEpi>())
+      if (st.issuer) tma_store_wait_read<0>();
   }
   if constexpr (kCM > 1) {
     __syncwarp();
@@ -368,10 +493,15 @@ static int num_sms() {
   return n;
 }
 
+// The operands' tensor maps and, for bf16 outputs, those of the epilogue's tensors (64 x 64 boxes); maps a variant does
+// not use stay zero.
+struct GemmMaps {
+  CUtensorMap a, b, out, aux, res;
+};
+
 template <int kBN, bool kAMN, bool kBMN, int kCM, int kEpi>
-static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const GemmArgs& args, int max_ctas,
-                       cudaStream_t stream) {
-  constexpr int kSmem = gemm_smem_bytes<kBN>();
+static int launch_gemm(const GemmMaps& maps, const GemmArgs& args, int max_ctas, cudaStream_t stream) {
+  constexpr int kSmem = gemm_smem_bytes<kBN, kEpi>();
   static int max_clusters = 0;
   auto kern = gemm_bf16_wgmma_kernel<kBN, kAMN, kBMN, kCM, kEpi>;
   cudaLaunchConfig_t cfg = {};
@@ -401,11 +531,11 @@ static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const GemmA
   if (max_ctas > 0 && clusters > max_ctas / kCM) clusters = max_ctas / kCM;
   if (clusters < 1) clusters = 1;
   cfg.gridDim = dim3(clusters * kCM);
-  if (cudaLaunchKernelEx(&cfg, kern, ta, tb, args) != cudaSuccess) return -30;
+  if (cudaLaunchKernelEx(&cfg, kern, maps.a, maps.b, maps.out, maps.aux, maps.res, args) != cudaSuccess) return -30;
   return cudaPeekAtLastError() == cudaSuccess ? 0 : -30;
 }
 
-typedef int (*LaunchFn)(const CUtensorMap&, const CUtensorMap&, const GemmArgs&, int, cudaStream_t);
+typedef int (*LaunchFn)(const GemmMaps&, const GemmArgs&, int, cudaStream_t);
 
 struct GemmKernel {
   bool a_mn, b_mn;
@@ -469,7 +599,11 @@ int aitj_gemm_bf16(const void* A, const void* B, void* out, int M, int N, int K,
   using namespace aitj;
   if (M <= 0 || N <= 0 || K <= 0) return 0;
   if ((N & 7) || (ldc & 7) || (lda & 7) || (ldb & 7)) return -1;
-  if ((reinterpret_cast<uintptr_t>(out) & 15) || ((flags & EPI_SAVE_PRE) && (reinterpret_cast<uintptr_t>(aux) & 15))) return -4;
+  // TMA needs 16-byte aligned tensors
+  if ((reinterpret_cast<uintptr_t>(out) & 15) ||
+      ((flags & (EPI_SAVE_PRE | EPI_DGELU)) && (reinterpret_cast<uintptr_t>(aux) & 15)) ||
+      ((flags & EPI_RESIDUAL) && (reinterpret_cast<uintptr_t>(residual) & 15)))
+    return -4;
   if (split_k > 1 && !(flags & EPI_ACCUM)) return -2;
   if ((flags & (EPI_MC | EPI_PEER)) && !(flags & EPI_ACCUM)) return -5;
   const int cm = block_n == 1024 ? 4 : (block_n == 512 ? 2 : 1);
@@ -502,15 +636,22 @@ int aitj_gemm_bf16(const void* A, const void* B, void* out, int M, int N, int K,
     if (k.a_mn == (a_mn != 0) && k.b_mn == (b_mn != 0) && k.epi == epi && k.block_n == block_n && k.cm == cm) kernel = &k;
   if (!kernel) return -7;
 
-  CUtensorMap ta, tb;
+  GemmMaps maps;
+  memset(&maps, 0, sizeof(maps));
   int rc;
-  if (!a_mn) rc = encode_2d(&ta, A, K, M, lda, BLOCK_K, BLOCK_M);
-  else       rc = encode_2d(&ta, A, M, K, lda, 64, BLOCK_K);
+  if (!a_mn) rc = encode_2d(&maps.a, A, K, M, lda, BLOCK_K, BLOCK_M);
+  else       rc = encode_2d(&maps.a, A, M, K, lda, 64, BLOCK_K);
   if (rc) return rc;
-  if (!b_mn) rc = encode_2d(&tb, B, K, N, ldb, BLOCK_K, block_n / cm);
-  else       rc = encode_2d(&tb, B, N, K, ldb, 64, BLOCK_K);
+  if (!b_mn) rc = encode_2d(&maps.b, B, K, N, ldb, BLOCK_K, block_n / cm);
+  else       rc = encode_2d(&maps.b, B, N, K, ldb, 64, BLOCK_K);
   if (rc) return rc - 1000;
-  rc = kernel->launch(ta, tb, args, max_ctas, stream);
+  if (!(flags & (EPI_OUT_F32 | EPI_ACCUM))) {
+    rc = encode_2d(&maps.out, out, N, M, ldc, 64, 64);
+    if (!rc && (flags & (EPI_SAVE_PRE | EPI_DGELU))) rc = encode_2d(&maps.aux, aux, N, M, ldc, 64, 64);
+    if (!rc && (flags & EPI_RESIDUAL)) rc = encode_2d(&maps.res, residual, N, M, ldc, 64, 64);
+    if (rc) return rc - 2000;
+  }
+  rc = kernel->launch(maps, args, max_ctas, stream);
   if (rc || !peer_move) return rc;
   const size_t nvec = static_cast<size_t>(M) * (N / 4);
   int blocks = static_cast<int>((nvec + 255) / 256);

@@ -21,6 +21,8 @@ EPI_MC = 128
 EPI_PEER = 16384
 EPI_COLSUM = 256   # set by the library when a colsum buffer is given
 
+# aitj_gemm_bf16: out, aux or residual is not 16-byte aligned (the epilogue reaches them by TMA)
+GEMM_MISALIGNED = -4
 # aitj_gemm_bf16: no kernel is compiled for this operand layout and epilogue
 GEMM_NO_KERNEL = -7
 

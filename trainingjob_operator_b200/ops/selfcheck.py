@@ -151,6 +151,65 @@ def case_gemm_epilogue():
         ok &= _check(f"peer wgrad split_k={sk_peer}: other rows at the owner", hi[half:], ref[half:], 1e-2)
         ok &= bool((lo[half:] == 0).all()) and bool((hi[:half] == 0).all())
     torch.cuda.synchronize()
+    return ok & _gemm_epilogue_tails()
+
+
+def _gemm_epilogue_tails():
+    """Every epilogue of the GPT-2 / BERT step, in all four tile configurations, with M and N tails that are not
+    multiples of 64 and out / aux / residual rows `ldc` > N apart.  The bf16 epilogues store whole 64 x 64 boxes by TMA,
+    clipped at N and M: the padding columns of every strided tensor must keep their sentinel."""
+    ok = True
+    M, N, K, ldc = 1000, 904, 328, 1032
+    a, b_nk, b_kn = _rand(M, K), _rand(N, K, scale=0.05), _rand(K, N, scale=0.05)
+    bias = _rand(N)
+    sentinel = 7.0
+
+    def strided(init=None):
+        buf = torch.full((M, ldc), sentinel, device="cuda", dtype=torch.bfloat16)
+        if init is not None:
+            buf[:, :N] = init
+        return buf, buf[:, :N]
+
+    _, res = strided(_rand(M, N))
+    _, pre = strided(_rand(M, N))
+    pf = pre.float().requires_grad_(True)
+    (gp,) = torch.autograd.grad(torch.nn.functional.gelu(pf, approximate="tanh").sum(), pf)
+    fwd = a.float() @ b_nk.float().t()
+    dgr = a.float() @ b_kn.float()
+    for bn in (128, 256, 512, 1024):
+        cases = [  # (name, b_mn, kwargs, reference, reference of the saved pre-activation)
+            ("fwd", False, {}, fwd, None),
+            ("fwd bias", False, {"bias": bias}, fwd + bias.float(), None),
+            ("fwd bias+gelu+save_pre", False, {"bias": bias, "gelu": True, "save_pre": True},
+             torch.nn.functional.gelu(fwd + bias.float(), approximate="tanh"), fwd + bias.float()),
+            ("fwd bias+residual", False, {"bias": bias, "residual": res}, fwd + bias.float() + res.float(), None),
+            ("dgrad", True, {}, dgr, None),
+            ("dgrad dgelu", True, {"dgelu": True, "aux": pre}, dgr * gp, None),
+            ("dgrad dgelu+colsum", True, {"dgelu": True, "aux": pre, "colsum": True}, dgr * gp, None),
+            ("dgrad residual", True, {"residual": res}, dgr + res.float(), None),
+        ]
+        for name, b_mn, kw, ref, pre_ref in cases:
+            kw = dict(kw)
+            obuf, out = strided()
+            abuf = None
+            if pre_ref is not None:
+                abuf, kw["aux"] = strided()
+            cs = None
+            if kw.get("colsum"):
+                cs = torch.full((N,), 2.0, device="cuda")
+                kw["colsum"] = cs
+            F.gemm(a, b_kn if b_mn else b_nk, out, b_mn=b_mn, block_n=bn, **kw)
+            torch.cuda.synchronize()
+            tag = f"bn={bn} M={M} N={N} ldc={ldc} {name}"
+            ok &= _check(tag, out, ref, 2e-2 if "dgelu" in name else 1e-2)
+            if pre_ref is not None:
+                ok &= _check(tag + ": saved pre-activation", kw["aux"], pre_ref, 1e-2)
+            if cs is not None:
+                ok &= _check(tag + ": column sums", cs, out.float().sum(0) + 2.0, 1e-3)
+            for buf in (obuf, abuf):
+                if buf is not None and not bool((buf[:, N:] == sentinel).all()):
+                    print(f"  {tag}: FAIL, a store reached the padding columns N..ldc", flush=True)
+                    ok = False
     return ok
 
 
