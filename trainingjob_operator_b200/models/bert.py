@@ -22,8 +22,8 @@ from typing import List, Tuple
 import torch
 import torch.nn.functional as TF
 
+from .engine import TransformerEngine
 from .flat_params import FlatParams, ParamSpec
-from .gpt2 import GPT2Engine, _LayerBufs
 
 MASK_TOKEN = 103
 
@@ -112,75 +112,28 @@ class SyntheticMLM:
         return b
 
 
-class _BertLayerBufs(_LayerBufs):
-    def __init__(self, M: int, C: int, dev):
-        super().__init__(M, C, dev)
-        self.out = torch.empty(M, C, device=dev, dtype=torch.bfloat16)     # x_{l+1} = LN2(res2); ln1 / ln2 hold y
-
-
-class BertEngine(GPT2Engine):
-    """Explicit forward / backward / optimizer of BERT-base MLM pre-training for a fixed (B, T) micro-batch on one GPU.
-    Reuses the GEMM front-ends, attention, optimizer and bucket logic of ``GPT2Engine``; the wiring is BERT's."""
+class BertEngine(TransformerEngine):
+    """Explicit forward / backward / optimizer of BERT-base MLM pre-training for a fixed (B, T) micro-batch on one GPU,
+    on ``TransformerEngine``.  Layer i's LN2 output, ``layers[i].ln2``, is the input of layer i + 1."""
 
     def __init__(self, cfg: BertConfig, batch_size: int, seq_len: int, device="cuda", seed: int = 0,
                  gemm_backend: str = "wgmma"):
-        from ..ops import functional as F
-        import os
-
-        assert seq_len <= cfg.block_size and cfg.n_embd % 256 == 0
-        self.F = F
-        self.cfg = cfg
-        self.B, self.T = batch_size, seq_len
-        self.M = batch_size * seq_len
-        self.dev = torch.device(device)
-        self.backend = gemm_backend
-        self.causal = False
-        self.attn_impl = os.environ.get("AITJ_ATTN", "cudnn")
-        if self.attn_impl == "wgmma" and (seq_len % 128 or cfg.n_embd // cfg.n_head != 64 or gemm_backend != "wgmma"):
-            self.attn_impl = "cudnn"
-        self.attn_bwd_impl = os.environ.get("AITJ_ATTN_BWD", "cudnn") if self.attn_impl == "wgmma" else "cudnn"
-        self._attn_delta = None
-        self._dq_acc = None
-        self._philox = torch.zeros((), dtype=torch.int64, device=device)
-        self.bwd_max_ctas = 0
-        self.params = FlatParams(bert_param_specs(cfg), self.dev, seed=seed)
-        C, M, Vp = cfg.n_embd, self.M, cfg.padded_vocab
-        with torch.no_grad():
-            self.params.w32("wte")[cfg.vocab_size:].zero_()
-            self.params.refresh_compute_copy()
+        super().__init__(cfg, bert_param_specs(cfg), batch_size, seq_len, device, seed, gemm_backend, causal=False,
+                         doc_mask=False)
+        C, M = cfg.n_embd, self.M
         bf = dict(device=self.dev, dtype=torch.bfloat16)
         f32 = dict(device=self.dev, dtype=torch.float32)
-        self.tok = torch.zeros(M, dtype=torch.int64, device=self.dev)
         self.typ = torch.zeros(M, dtype=torch.int64, device=self.dev)
-        self.tgt = torch.full((M,), -1, dtype=torch.int64, device=self.dev)
+        self.tgt.fill_(-1)
         self.n_masked = max(1, int(round(0.15 * M)))
         self.e0 = torch.empty(M, C, **bf)                      # sum of the three embeddings
         self.x0 = torch.empty(M, C, **bf)                      # LN(e0): input of layer 0
         self.e_mean, self.e_rstd = torch.empty(M, **f32), torch.empty(M, **f32)
-        self.layers = [_BertLayerBufs(M, C, self.dev) for _ in range(cfg.n_layer)]
         self.mlm_pre = torch.empty(M, C, **bf)
         self.mlm_act = torch.empty(M, C, **bf)
         self.mlm_ln = torch.empty(M, C, **bf)
         self.m_mean, self.m_rstd = torch.empty(M, **f32), torch.empty(M, **f32)
-        self.logits = torch.empty(M, Vp, **bf)
-        self.losses = torch.empty(M, **f32)
-        self.loss = torch.zeros(1, **f32)
         self.d_x = [torch.empty(M, C, **bf) for _ in range(3)]
-        self.d_fc = torch.empty(M, 4 * C, **bf)
-        self.d_qkv = torch.empty(M, 3 * C, **bf)
-        self.d_att = torch.empty(M, C, **bf)
-        self.sumsq = torch.zeros(1, **f32)
-        self.dyn = torch.zeros(4, **f32)
-        self._dyn_host = torch.zeros(4, dtype=torch.float32).pin_memory() if self.dev.type == "cuda" else None
-        self.pair = os.environ.get("AITJ_GEMM_PAIR", "1") != "0"
-        self.gemm_cfg = {}
-        self.wgrad_stream = torch.cuda.Stream() if (self.dev.type == "cuda" and gemm_backend == "wgmma" and
-                                                    os.environ.get("AITJ_WGRAD_STREAM", "0") != "0") else None
-        self._wgrad_done = None
-        self.segment_join = False
-        self.grad_hook = None
-        self._graph = None
-        self.split_k = {}
 
     def input_tensors(self) -> List[torch.Tensor]:
         return [self.tok, self.typ, self.tgt]
@@ -188,7 +141,7 @@ class BertEngine(GPT2Engine):
     # ------------------------------------------------------------------ forward
     @torch.no_grad()
     def forward(self) -> torch.Tensor:
-        F, P, cfg = self.F, self.params, self.cfg
+        F, P = self.F, self.params
         F.embedding3_fwd(self.tok, self.typ, P.w16("wte"), P.w16("wpe"), P.w16("wtt"), self.e0, self.T)
         F.layernorm_fwd(self.e0, P.w16("emb_ln_w"), P.w16("emb_ln_b"), self.x0, self.e_mean, self.e_rstd)
         x = self.x0
@@ -200,30 +153,20 @@ class BertEngine(GPT2Engine):
             F.layernorm_fwd(lb.res1, P.w16(p + "ln1_w"), P.w16(p + "ln1_b"), lb.ln1, lb.ln1_mean, lb.ln1_rstd)      # y
             self._linear(lb.ln1, P.w16(p + "fc_w"), lb.fc_act, bias=P.w16(p + "fc_b"), gelu=True, aux=lb.fc_pre)
             self._linear(lb.fc_act, P.w16(p + "fc2_w"), lb.res2, bias=P.w16(p + "fc2_b"), residual=lb.ln1)
-            F.layernorm_fwd(lb.res2, P.w16(p + "ln2_w"), P.w16(p + "ln2_b"), lb.out, lb.ln2_mean, lb.ln2_rstd)
-            x = lb.out
+            F.layernorm_fwd(lb.res2, P.w16(p + "ln2_w"), P.w16(p + "ln2_b"), lb.ln2, lb.ln2_mean, lb.ln2_rstd)
+            x = lb.ln2
         # MLM head: dense + GELU + LayerNorm, decoder tied to the word embeddings (+ its own bias)
         self._linear(x, P.w16("mlm_w"), self.mlm_act, bias=P.w16("mlm_b"), gelu=True, aux=self.mlm_pre)
         F.layernorm_fwd(self.mlm_act, P.w16("mlm_ln_w"), P.w16("mlm_ln_b"), self.mlm_ln, self.m_mean, self.m_rstd)
         self._linear(self.mlm_ln, P.w16("wte"), self.logits, bias=P.w16("dec_b"))
-        F.softmax_xent(self.logits, self.tgt, self.losses, cfg.vocab_size, 1.0 / self.n_masked)
-        torch.sum(self.losses, dim=0, keepdim=True, out=self.loss)
-        self.loss.mul_(1.0 / self.n_masked)
-        return self.loss
+        return self._loss(self.n_masked)
 
-    # ------------------------------------------------------------------ backward
-    def backward_segments(self):
-        segs = [((), self._bwd_head)]
-        for i in range(len(self.layers) - 1, -1, -1):
-            segs.append(((f"h{i}",), (lambda i=i: self._bwd_layer(i))))
-        segs.append((("emb", "small"), self._bwd_tail))
-        return segs
-
+    # ------------------------------------------------------------------ backward segments
     @torch.no_grad()
     def _bwd_head(self) -> None:
         F, P = self.F, self.params
         dlogits = self.logits
-        x_last = self.layers[-1].out if self.layers else self.x0
+        x_last = self.layers[-1].ln2 if self.layers else self.x0
         d_t, d_g, d_u = self.d_x
         F.colsum(dlogits, P.grad("dec_b"))
         self._dgrad(dlogits, P.w16("wte"), d_t)
@@ -243,7 +186,7 @@ class BertEngine(GPT2Engine):
         F, P = self.F, self.params
         lb = self.layers[i]
         p = f"h{i}."
-        x_in = self.layers[i - 1].out if i > 0 else self.x0
+        x_in = self.layers[i - 1].ln2 if i > 0 else self.x0
         self._join_wgrads()                                  # last segment's weight gradients still read these buffers
         free = [t for t in self.d_x if t is not self._d_cur]
         d_r, d_y = free

@@ -97,23 +97,22 @@ class EngineTrainer:
         if self.world > 1 and self.symm is None and self.shard is None:
             self.reducer = BucketAllReducer(engine.params.g32, engine.grad_buckets(), group, backend)
         engine.grad_hook = self.reducer.hook if self.reducer else None
-        if self.reducer is not None and hasattr(engine, "bwd_max_ctas"):
+        if self.reducer is not None:
             reserve = int(os.environ.get("AITJ_DDP_RESERVE_SMS", "0"))
             if reserve > 0:
                 from ..ops import functional as F
 
                 engine.bwd_max_ctas = max(2, (F.num_sms() - reserve) // 2 * 2)
-                engine.split_k.clear() if hasattr(engine, "split_k") else None
+                engine.split_k.clear()
         # Without library collectives (1 GPU, or the fused multicast path) the whole step is ONE CUDA graph.  With
         # the NCCL reducer the step is a chain of graphs split where a gradient bucket becomes final; the bucket's
         # all-reduce is launched between two replays on the side stream (capturing NCCL itself deadlocked on
         # the 2-GPU box), so collectives overlap the next segment's math and nothing else is launched eagerly.
         self.use_graph = use_graph and self.cuda
         self.segmented = self.reducer is not None
-        if hasattr(engine, "segment_join"):
-            # NCCL mode: a bucket's all-reduce starts when its segment's kernels are done, and segments are separate
-            # graphs -- each one joins the weight-gradient side stream at its end
-            engine.segment_join = self.segmented
+        # NCCL mode: a bucket's all-reduce starts when its segment's kernels are done, and segments are separate
+        # graphs -- each one joins the weight-gradient side stream at its end
+        engine.segment_join = self.segmented
         self.seg_graphs = None
         self.graph: Optional[torch.cuda.CUDAGraph] = None
         self.loss_host = torch.zeros(1, dtype=torch.float32)
