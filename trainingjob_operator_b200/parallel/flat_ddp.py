@@ -73,6 +73,11 @@ class FlatDDP:
         self.reducer = BucketAllReducer(self.g32, buckets, group, backend, min_bucket_bytes=0) \
             if self.world > 1 else None
         self._hooked = False
+        # micro-batch accumulation: ``k`` micro-batches per optimizer step, whole job (None: one per rank, k = world);
+        # ``sync`` is cleared while a rank runs a micro-batch that is not its last of the step, so that the bucket hooks
+        # leave the partial sums alone
+        self.k = None
+        self.sync = True
         if self.reducer is not None and overlap:
             for idx, p in enumerate(params):
                 p.register_post_accumulate_grad_hook(self._make_hook(idx))
@@ -83,7 +88,7 @@ class FlatDDP:
         b = self._bucket_of[idx]
 
         def hook(_p):
-            if self.reducer is None:
+            if self.reducer is None or not self.sync:
                 return
             self._todo[b] -= 1
             if self._todo[b] == 0:
@@ -112,17 +117,19 @@ class FlatDDP:
         self.g32.zero_()
 
     def step(self) -> None:
-        """Fused optimizer sweep (+ gradient zeroing); grads are averaged over the world size."""
+        """Fused optimizer sweep (+ gradient zeroing); the summed gradients are divided by the number of micro-batches of
+        the step, whole job (the world size without accumulation): a mean of per-micro-batch mean gradients."""
         self.step_count += 1
+        div = float(self.k or self.world)
         if self.dev.type == "cuda" and self.optimizer == "adamw":
             from ..ops import functional as F
 
             F.adamw(self.p32, self.g32, self.m, self.v, self.p16, self.wd_mask, lr=self.lr, beta1=0.9, beta2=0.999,
-                    eps=1e-8, weight_decay=self.weight_decay, step=self.step_count, grad_div=float(self.world),
+                    eps=1e-8, weight_decay=self.weight_decay, step=self.step_count, grad_div=div,
                     zero_grad=True)
             return
         with torch.no_grad():
-            g = self.g32 / float(self.world)
+            g = self.g32 / div
             if self.optimizer == "adamw":
                 b1, b2 = 0.9, 0.999
                 self.m.mul_(b1).add_(g, alpha=1 - b1)

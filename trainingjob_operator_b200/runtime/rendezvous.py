@@ -270,10 +270,34 @@ class StallBreaker:
         # how long one step may take before it counts as stuck: ``after_s``, except for the first step after a (re-)bind,
         # which legitimately takes seconds (kernel loading, CUDA-graph capture) -- the worker raises it for that step
         self.patience = after_s
+        self._measured_generation = None    # generation whose steps the patience follows (begin_step / step_done)
+        self._first_step = 0.0
+        self._slowest_steady: Optional[float] = None
         self.tripped = False
         self._stop = threading.Event()
         self._t = threading.Thread(target=self._run, name="stall-breaker", daemon=True)
         self._t.start()
+
+    FIRST_STEP_S = 30.0     # patience for the first step on a freshly bound trainer (kernel loading, graph capture)
+
+    def begin_step(self, generation: int) -> None:
+        """At a step boundary: the patience for the coming step, from the steps this generation has completed.  None yet:
+        ``FIRST_STEP_S``.  Only the first: twice that step -- it did everything a steady step does and also loaded
+        kernels and captured graphs, so it bounds a steady step from above.  Otherwise twice the slowest steady step -- a
+        step that accumulates many micro-batches legitimately takes seconds.  Never less than ``after_s``."""
+        if self._measured_generation != generation:
+            self.patience = max(self.after_s, self.FIRST_STEP_S)
+        elif self._slowest_steady is None:
+            self.patience = max(self.after_s, 2.0 * self._first_step)
+        else:
+            self.patience = max(self.after_s, 2.0 * self._slowest_steady)
+
+    def step_done(self, generation: int, seconds: float) -> None:
+        """A training step of ``generation`` completed in ``seconds``."""
+        if self._measured_generation != generation:
+            self._measured_generation, self._first_step, self._slowest_steady = generation, seconds, None
+        else:
+            self._slowest_steady = max(self._slowest_steady or 0.0, seconds)
 
     def progress(self, generation: int) -> None:
         self.generation = generation

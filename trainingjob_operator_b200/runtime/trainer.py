@@ -3,8 +3,9 @@ bucketed gradient all-reduce overlapped with backward, fused optimizer sweep, lo
 
 One ``step()`` is exactly what BASELINE.json's samples/sec counts and what ``bench.py`` times:
 H2D copy of this step's tokens from pinned memory -> forward -> backward (+ all-reduce) ->
-AdamW -> D2H of the loss.  The reference operator has no training loop (SURVEY.md §2.6); this is the
-launched workers' loop.
+AdamW -> D2H of the loss.  With a global batch of several micro-batches per rank (``runtime/accumulation.py``),
+``accumulate()`` runs forward + backward for every micro-batch but the last, then that step.  The reference operator
+has no training loop (SURVEY.md §2.6); this is the launched workers' loop.
 """
 from __future__ import annotations
 
@@ -17,6 +18,7 @@ import torch
 import torch.distributed as dist
 
 from ..parallel.ddp import BucketAllReducer
+from .accumulation import micro_batch_plan
 
 
 class SyntheticTokens:
@@ -49,7 +51,9 @@ def cosine_lr(step: int, base_lr: float, warmup: int = 10, total: int = 10000, m
 
 class EngineTrainer:
     def __init__(self, engine, lr: float = 3e-4, weight_decay: float = 0.1, max_norm: float = 1.0,
-                 use_graph: bool = True, allreduce: Optional[str] = None, group=None):
+                 use_graph: bool = True, allreduce: Optional[str] = None, group=None, global_batch: int = 0):
+        """``global_batch``: samples per optimizer step for the whole job (0: world size x the engine's batch), trained
+        in micro-batches of the engine's batch as ``runtime.accumulation.micro_batch_plan`` assigns them."""
         self.engine = engine
         self.lr = lr
         self.weight_decay = weight_decay
@@ -58,6 +62,7 @@ class EngineTrainer:
         self.rank = dist.get_rank(group) if dist.is_initialized() else 0
         self.group = group
         self.step_count = 0
+        self.plan = micro_batch_plan(global_batch, engine.B, self.world, self.rank)
         self.cuda = engine.dev.type == "cuda"
         # rs (default): gradients are reduce-scattered to their owner rank by the kernels that produce them, over NVLink
         # peer memory; sharded AdamW; bf16 parameters all-gathered by multicast stores (parallel/symm.ShardedGradState).
@@ -82,6 +87,10 @@ class EngineTrainer:
             else:
                 self.allreduce_backend = f"nccl (rs unavailable: {sh.reason})"
                 backend = "nccl"
+        if self.world > 1 and backend == "mc" and self.cuda and self.plan.accumulates:
+            # the multicast path needs every peer at a barrier before each backward: it has no micro-batch step
+            raise ValueError("AITJ_ALLREDUCE=mc cannot accumulate micro-batches (global batch "
+                             f"{self.plan.global_batch} != {self.world} x {engine.B})")
         if self.world > 1 and backend == "mc" and self.cuda:
             # fused GEMM -> all-reduce: gradients are reduced through the NVSwitch multicast alias by the kernels
             # that produce them (parallel/symm.py); no gradient collective is launched at all
@@ -120,6 +129,10 @@ class EngineTrainer:
             self.loss_host = self.loss_host.pin_memory()
         self.graph_error: Optional[str] = None
         self.launches_per_step = 0
+        # micro-batch accumulation: the graphs of accumulate() in one-graph mode ("micro", "last" or "idle"), and the
+        # sum of this rank's micro-batch losses of the step, kept on the device until the step's one read-back
+        self.acc_graphs: Optional[dict] = None
+        self.loss_sum = torch.zeros(1, dtype=torch.float32, device=engine.dev)
 
     # ------------------------------------------------------------------ one step of device work
     def _device_step(self) -> None:
@@ -140,21 +153,165 @@ class EngineTrainer:
             self.shard.barrier()
 
     def _optimizer(self) -> None:
+        # the gradient buffers hold the sum over the job's k micro-batches of per-micro-batch mean gradients (k = the
+        # world size without accumulation)
         self.engine.optimizer_step(lr=self.lr, step=max(1, self.step_count), weight_decay=self.weight_decay,
-                                   max_norm=self.max_norm, grad_div=float(self.world), use_dyn=True)
+                                   max_norm=self.max_norm, grad_div=float(self.plan.k), use_dyn=True)
 
+    # ------------------------------------------------------------------ micro-batch accumulation
+    def _micro_step(self) -> None:
+        """A micro-batch that is not this rank's last of the step: forward + backward only, adding into the gradient
+        buffers (no bucket hooks, no collectives, no barriers, no optimizer)."""
+        e = self.engine
+        e.forward()
+        hook, e.grad_hook = e.grad_hook, None
+        try:
+            e.backward()
+        finally:
+            e.grad_hook = hook
+        self.loss_sum.add_(e.loss)
+
+    def _last_step(self) -> None:
+        """This rank's last micro-batch of the step: the single-micro-batch step (gradient sync + optimizer)."""
+        self._device_step()
+        self.loss_sum.add_(self.engine.loss)
+
+    def _idle_step(self, optimizer=None) -> None:
+        """A rank with no micro-batch in this step: the gradient sync and the optimizer of ``_device_step`` on its zero
+        gradient, so that it issues the same barriers and bucket all-reduces, in the same order, as the other ranks.
+        ``optimizer``: the optimizer's replay when the step runs as graph segments."""
+        e = self.engine
+        if self.shard is not None:
+            self.shard.barrier()
+        if self.reducer:
+            for buckets, _ in e.backward_segments():
+                for b in buckets:
+                    self.reducer.hook(b)
+            self.reducer.wait()
+        (optimizer or self._optimizer)()
+        if self.shard is not None:
+            self.shard.barrier()
+
+    def _eager_step(self) -> None:
+        """One complete optimizer step of this rank's micro-batches, launched eagerly on the current inputs."""
+        if self.plan.n == 0:
+            self._idle_step()
+            return
+        for _ in range(self.plan.n - 1):
+            self._micro_step()
+        self._last_step()
+
+    def _run(self, kind: str) -> None:
+        """``kind``: "micro", "last" or "idle" -- from the captured graphs when there are any."""
+        if self.seg_graphs is not None:
+            if kind == "micro":
+                for _, g in self.seg_graphs[:-1]:          # forward and backward segments; no hook, no optimizer
+                    g.replay()
+                self.loss_sum.add_(self.engine.loss)
+            elif kind == "last":
+                self._replay_segments()
+                self.loss_sum.add_(self.engine.loss)
+            else:
+                self._idle_step(self.seg_graphs[-1][1].replay)
+        elif self.acc_graphs is not None:
+            self.acc_graphs[kind].replay()
+        else:
+            {"micro": self._micro_step, "last": self._last_step, "idle": self._idle_step}[kind]()
+
+    def _warm_up(self) -> None:
+        """Two complete steps on a side stream before capture (allocator, cuDNN plans, NCCL channels).  With a fixed
+        global batch the state they updated is put back afterwards on every rank -- also at a world size where the step
+        is a single micro-batch (k = W): where a job captured its graphs (first step, every rescale) then leaves no mark
+        on the optimisation, whatever the world sizes it passes through."""
+        P = self.engine.params
+        snap = [t.clone() for t in P.state_tensors()] if self.plan.fixed else None
+        s = torch.cuda.Stream()
+        s.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(s):
+            for _ in range(2):
+                if snap is None:
+                    self._device_step()
+                else:
+                    self._eager_step()
+        torch.cuda.current_stream().wait_stream(s)
+        torch.cuda.synchronize()
+        if snap is not None:
+            # (every rank's state is whole here: the trainer was bound right before the state hand-off.  The last
+            # barrier of the warm-up ordered every peer's stores into this rank's bf16 copy before the refresh, and no
+            # peer stores into it again before the barrier inside the next optimizer sweep.)
+            for t, v in zip(P.state_tensors(), snap):
+                t.copy_(v)
+            P.refresh_compute_copy()
+            self.loss_sum.zero_()
+            torch.cuda.synchronize()
+
+    def _capture_accumulating(self) -> None:
+        """One-graph mode with accumulation: a graph per kind of micro-batch this rank runs -- "micro" (n >= 2) and
+        "last" (n >= 1), or "idle" (n = 0).  Capturing records; it does not execute."""
+        from ..ops import lib
+
+        n = self.plan.n
+        kinds = {"idle": self._idle_step} if n == 0 else \
+            dict(([("micro", self._micro_step)] if n >= 2 else []) + [("last", self._last_step)])
+        graphs, launches = {}, {}
+        try:
+            for kind, fn in kinds.items():
+                before = lib.LAUNCHES
+                g = torch.cuda.CUDAGraph()
+                with torch.cuda.graph(g):
+                    fn()
+                graphs[kind], launches[kind] = g, lib.LAUNCHES - before
+            self.acc_graphs = graphs
+            self.graph = graphs.get("last") or graphs["idle"]
+            self.launches_per_step = launches.get("idle", 0) + launches.get("last", 0) + \
+                launches.get("micro", 0) * max(0, n - 1)
+        except Exception as ex:  # noqa: BLE001 - fall back to eager launches
+            self.acc_graphs = self.graph = None
+            self.use_graph = False
+            self.graph_error = f"{type(ex).__name__}: {ex}"
+            torch.cuda.synchronize()
+
+    def accumulate(self, micro_inputs, read_loss: bool = True) -> Optional[float]:
+        """One optimizer step over this rank's ``plan.n`` micro-batches.  ``micro_inputs`` yields each micro-batch's
+        inputs in pinned host memory (as ``step`` takes them), and is drawn lazily: the next micro-batch is taken once
+        the previous one's copies and work are enqueued, and the iterator runs on after the last one.  Returns the mean
+        of this rank's micro-batch losses (NaN when it has none), read back once per step; nothing synchronises with
+        the host between micro-batches."""
+        e = self.engine
+        n = self.plan.n
+        self.step_count += 1
+        e.set_step_scalars(cosine_lr(self.step_count, self.lr), self.step_count)
+        captured = not self.use_graph or self.seg_graphs is not None or self.acc_graphs is not None
+        done = 0
+        for host in micro_inputs:
+            for dst, src in zip(e.input_tensors(), host):
+                dst.copy_(src, non_blocking=True)
+            if not captured:
+                self._capture_segments() if self.segmented else self._capture()
+                captured = True
+            self._run("micro" if done < n - 1 else "last")
+            done += 1
+        if done != n:
+            raise ValueError(f"rank {self.rank} runs {n} micro-batches per step, {done} were given")
+        if n == 0:
+            if not captured:
+                self._capture_segments() if self.segmented else self._capture()
+            self._run("idle")
+        if not read_loss:
+            return None
+        self.loss_host.copy_(self.loss_sum, non_blocking=True)
+        self.loss_sum.zero_()
+        if self.cuda:
+            torch.cuda.current_stream().synchronize()
+        return float(self.loss_host[0]) / n if n else float("nan")
+
+    # ------------------------------------------------------------------ graph capture
     def _capture_segments(self) -> None:
         """NCCL mode: [forward] [bwd head] [layer L-1] ... [layer 0] [tail] [optimizer] as separate graphs."""
         from ..ops import lib
 
         e = self.engine
-        s = torch.cuda.Stream()
-        s.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(s):
-            for _ in range(2):
-                self._device_step()
-        torch.cuda.current_stream().wait_stream(s)
-        torch.cuda.synchronize()
+        self._warm_up()
         saved_hook, e.grad_hook = e.grad_hook, None
         parts = [((), e.forward)] + list(e.backward_segments()) + [(None, self._optimizer)]
         graphs = []
@@ -189,14 +346,10 @@ class EngineTrainer:
     def _capture(self) -> None:
         from ..ops import lib
 
-        # warm-up on a side stream (allocator, cuDNN plans, NCCL channels) before capture
-        s = torch.cuda.Stream()
-        s.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(s):
-            for _ in range(2):
-                self._device_step()
-        torch.cuda.current_stream().wait_stream(s)
-        torch.cuda.synchronize()
+        self._warm_up()
+        if self.plan.accumulates:
+            self._capture_accumulating()
+            return
         before = lib.LAUNCHES
         g = torch.cuda.CUDAGraph()
         try:

@@ -89,17 +89,27 @@ class EngineAdapter:
         if hasattr(self, "data_position"):
             self.describe.update(data=args.data, doc_mask=self.engine.doc_mask, windows=self.data.n_windows)
 
-    def bind(self, group=None) -> None:
+    def bind(self, group=None, warm_up: bool = False) -> None:
+        """(Re-)build the trainer for the current process group; the micro-batch plan follows its world size.
+        ``warm_up``: a joiner's throw-away steps before it enters the job, one micro-batch each."""
         old = self.trainer
         # a faultTolerant job survives the loss of a peer in place, which needs every rank to hold the whole optimizer
         # state and a collective that can be aborted: library all-reduce instead of the owner-sharded peer-memory path
         allreduce = "nccl" if os.environ.get("AITJ_FAULT_TOLERANT") == "1" and "AITJ_ALLREDUCE" not in os.environ else None
         self.trainer = EngineTrainer(self.engine, lr=self.args.lr, use_graph=not self.args.no_graph, group=group,
-                                     allreduce=allreduce)
+                                     allreduce=allreduce,
+                                     global_batch=0 if warm_up else getattr(self.args, "global_batch", 0))
         if old is not None:
             self.trainer.step_count = old.step_count
 
+    @property
+    def plan(self):
+        return self.trainer.plan
+
     def train_step(self) -> float:
+        plan = getattr(self.trainer, "plan", None)
+        if plan is not None and plan.accumulates:
+            return self.trainer.accumulate(self._micro_inputs())
         if not hasattr(self, "data_position"):
             return self.trainer.step(*self.data.next())
         world, rank = self.trainer.world, self.trainer.rank
@@ -109,10 +119,30 @@ class EngineAdapter:
         self.data_position += world * self.batch     # not reached when the step fails: a discarded step reads again
         return loss
 
+    def _micro_inputs(self):
+        """This rank's micro-batches of the step, staged one at a time as the trainer takes them; the data position moves
+        by the global batch once the last one is enqueued.  Without ``--data`` each takes the next synthetic batch."""
+        plan = self.trainer.plan
+        if not hasattr(self, "data_position"):
+            for _ in range(plan.n):
+                yield self.data.next()
+                heartbeat()
+            return
+        read = []
+        for first, count in plan.windows(self.data_position):
+            yield self.data.stage(first, count)
+            self.data.in_flight()
+            read += self.data.samples_read
+            heartbeat()                    # a long accumulated step must not look like a hang to the agent
+        self.samples_read = read
+        self.data_position += plan.global_batch
+
     def discard_step(self) -> None:
         self.engine.params.g32.zero_()
         if self.engine.params.g_small is not None:
             self.engine.params.g_small.zero_()
+        if self.trainer is not None:
+            self.trainer.loss_sum.zero_()
 
     def prepare_state(self) -> None:
         """Collective.  With the owner-sharded optimizer every rank only keeps its own range of the fp32 master weights
@@ -196,9 +226,11 @@ class TorchAdapter:
         self.loss_host = torch.zeros(1).pin_memory() if pin else torch.zeros(1)
         self.describe = {"model": name, "params": sum(p.numel() for p in self.module.parameters())}
         self.flops_per_step = 0.0
+        self.use_graph, self.graph, self.graph_error = False, None, None
 
-    def bind(self, group=None) -> None:
+    def bind(self, group=None, warm_up: bool = False) -> None:
         from ..parallel.flat_ddp import FlatDDP
+        from .accumulation import micro_batch_plan
 
         backend = "nccl" if self.dev.type == "cuda" else "gloo"
         # CUDA: forward + backward are replayed as one CUDA graph (the step of the small networks is launch bound: MNIST
@@ -218,6 +250,10 @@ class TorchAdapter:
                 for idx, p in enumerate(self.ddp.params):
                     p.register_post_accumulate_grad_hook(self.ddp._make_hook(idx))
         self.ddp._hooked = self.ddp.reducer is not None or getattr(self.ddp, "_hooked", False)
+        world = self.ddp.world
+        rank = dist.get_rank(group) if dist.is_initialized() else 0
+        self.plan = micro_batch_plan(0 if warm_up else getattr(self.args, "global_batch", 0), self.batch, world, rank)
+        self.ddp.k = self.plan.k
 
     def _fwd_bwd(self) -> torch.Tensor:
         if self.dev.type == "cuda":
@@ -251,26 +287,49 @@ class TorchAdapter:
             self.use_graph = False
             torch.cuda.synchronize()
 
-    def train_step(self) -> float:
-        x, y = self.batches[self.i % len(self.batches)]
+    def _batch(self, j: int):
+        """Synthetic inputs of micro-batch ``j``.  With a fixed global batch micro-batch j of step s takes batch s*k + j
+        of the cycle, so the job's batches do not depend on the world size; otherwise each rank cycles its own."""
+        if self.plan.fixed:
+            return self.batches[(self._steps * self.plan.k + j) % len(self.batches)]
+        b = self.batches[self.i % len(self.batches)]
         self.i += 1
-        self.x_dev.copy_(x, non_blocking=True)
-        self.y_dev.copy_(y, non_blocking=True)
-        if getattr(self, "use_graph", False) and getattr(self, "graph", None) is None and \
-                getattr(self, "graph_error", None) is None:
-            self._capture()
-        if getattr(self, "graph", None) is not None:
-            self.graph.replay()
-            loss = self._graph_loss
-        else:
-            loss = self._fwd_bwd()
+        return b
+
+    def train_step(self) -> float:
+        """One optimizer step over this rank's micro-batches (one without ``--global-batch``): forward + backward of each
+        adds into the flat gradient buffer -- the bucket hooks held back until the last one -- then one gradient
+        reduction and one optimizer sweep.  A rank without micro-batches reduces its zero buffer."""
+        n = self.plan.n
+        loss_sum = None
+        for j, mb in enumerate(self.plan.micro):
+            x, y = self._batch(mb)
+            self.x_dev.copy_(x, non_blocking=True)
+            self.y_dev.copy_(y, non_blocking=True)
+            if self.use_graph and self.graph is None and self.graph_error is None:
+                self._capture()
+            self.ddp.sync = j == n - 1
+            try:
+                if self.graph is not None:
+                    self.graph.replay()
+                    loss = self._graph_loss
+                else:
+                    loss = self._fwd_bwd()
+            finally:
+                self.ddp.sync = True
+            loss = loss.detach().float()
+            loss_sum = loss if loss_sum is None else loss_sum + loss
+            if n > 1:
+                heartbeat()               # a long accumulated step must not look like a hang to the agent
         self.ddp.finish_backward()
         self.ddp.step()
         self._steps += 1
-        self.loss_host.copy_(loss.detach().float().reshape(1), non_blocking=True)
+        if loss_sum is None:
+            return float("nan")
+        self.loss_host.copy_(loss_sum.reshape(1), non_blocking=True)
         if self.dev.type == "cuda":
             torch.cuda.current_stream().synchronize()
-        return float(self.loss_host[0])
+        return float(self.loss_host[0]) / n
 
     def discard_step(self) -> None:
         if self.ddp is not None:
@@ -421,7 +480,7 @@ def run(args) -> Dict[str, Any]:
         # Joining a running job: do everything that needs no peer first -- CUDA context, model build, two throw-away
         # steps (kernel loading, cuDNN plans, allocator growth; the state is overwritten by rank 0's broadcast
         # anyway) -- and only then tell the survivors, who keep training until this rank is ready to rendezvous.
-        adapter.bind(None)
+        adapter.bind(None, warm_up=True)     # single-micro-batch steps: not 2k micro-batches of throw-away work
         for _ in range(2):
             adapter.train_step()
         if use_cuda:
@@ -486,7 +545,6 @@ def run(args) -> Dict[str, Any]:
     timed_from = -1          # first step inside the timed region (-1: not armed yet)
     step = joined_step
     first_step_done = False
-    warmed_generation = -1          # generation whose trainer has completed at least one step
     pending_rescale = None
     from ..ops import lib as oplib
 
@@ -497,8 +555,9 @@ def run(args) -> Dict[str, Any]:
     while step < total and not stop["flag"]:
         if breaker is not None:
             breaker.progress(generation)
-            # the first step on a freshly bound trainer captures CUDA graphs / loads kernels: seconds, not a stall
-            breaker.patience = breaker.after_s if warmed_generation == generation else max(breaker.after_s, 30.0)
+            # patience from this generation's completed steps: the first step on a freshly bound trainer captures CUDA
+            # graphs / loads kernels, and an accumulated step can take seconds -- neither is a stall
+            breaker.begin_step(generation)
         failure = None
         try:
             # ---- elastic: agree on the newest rendezvous generation at the step boundary ------------
@@ -551,12 +610,14 @@ def run(args) -> Dict[str, Any]:
             if breaker is not None:
                 breaker.progress(generation)
                 breaker.in_step = True
+            t_step = time.perf_counter()
             try:
                 loss = adapter.train_step()
             finally:
                 if breaker is not None:
                     breaker.in_step = False
-            warmed_generation = generation
+            if breaker is not None:
+                breaker.step_done(generation, time.perf_counter() - t_step)
             if breaker is not None and breaker.tripped:
                 raise RuntimeError("the communicator was aborted while this step was in flight")
         except RuntimeError as e:
@@ -657,9 +718,10 @@ def run(args) -> Dict[str, Any]:
         if rank == 0 and watcher is not None and report_every > 0 and time.time() - live_t0 >= report_every:
             dt, n = time.time() - live_t0, step - live_step0
             if n > 0:
-                watcher.report_live(rank, {"samples_per_sec": round(args.batch * world * n / dt, 2),
+                G = adapter.plan.global_batch
+                watcher.report_live(rank, {"samples_per_sec": round(G * n / dt, 2),
                                            "ms_per_step": round(dt * 1e3 / n, 3), "world": world, "steps_done": step,
-                                           "global_batch": args.batch * world, "recoveries": len(recoveries)})
+                                           "global_batch": G, "recoveries": len(recoveries)})
             live_t0, live_step0 = time.time(), step
         if args.ckpt_every > 0 and step % args.ckpt_every == 0:
             adapter.prepare_state()
@@ -688,7 +750,8 @@ def run(args) -> Dict[str, Any]:
         wall = time.perf_counter() - t_wall0
         dev_ms = ev0.elapsed_time(ev1) if use_cuda else wall * 1e3
         dev_ms = max_over_ranks(dev_ms, device)
-        global_batch = args.batch * world
+        plan = adapter.plan
+        global_batch = plan.global_batch
         result.update({"timed_steps": n_timed, "timed_from_step": timed_from,
                        "timed_region_epoch": [t_epoch0, t_epoch1]})
         graph_launches = adapter.launches_per_step()
@@ -698,11 +761,12 @@ def run(args) -> Dict[str, Any]:
             "samples_per_sec": global_batch * n_timed / (dev_ms / 1e3),
             "wall_ms_per_step": wall * 1e3 / n_timed,
             "global_batch": global_batch, "batch_per_gpu": args.batch,
+            "micro_batches": plan.k, "micro_batches_this_rank": plan.n,
             "h2d_bytes_per_step": adapter.h2d_bytes, "d2h_bytes_per_step": adapter.d2h_bytes,
             "gpu_launches": graph_launches * n_timed if graph_launches else eager_launches,
             "launches_per_step": graph_launches or (eager_launches // max(1, n_timed)),
             "loss_first": losses[0] if losses else None, "loss_last": losses[-1] if losses else None,
-            "flops_per_step": getattr(adapter, "flops_per_step", 0.0),
+            "flops_per_step": getattr(adapter, "flops_per_step", 0.0) * plan.n,     # this rank's work
             "describe": adapter.describe,
             "cuda_graph": bool(getattr(getattr(adapter, "trainer", None), "graph", None)
                                or getattr(getattr(adapter, "trainer", None), "seg_graphs", None)
@@ -758,7 +822,15 @@ def parse_args(argv=None):
                     help="with --data: a token attends only to earlier tokens of its own document (documents start at "
                          "the end-of-text token); runs the wgmma attention kernels")
     ap.add_argument("--eot-token", type=int, default=50256, help="end-of-text token id that starts a document")
+    ap.add_argument("--global-batch", type=int, default=0, metavar="G",
+                    help="samples per optimizer step for the whole job, at any world size: each step trains G / --batch "
+                         "micro-batches, spread over the ranks, and sums their gradients (0 = world size x --batch)")
     args = ap.parse_args(argv)
+    if args.global_batch < 0 or args.global_batch % args.batch:
+        ap.error(f"--global-batch {args.global_batch} is not a multiple of --batch {args.batch}")
+    if args.global_batch and os.environ.get("AITJ_ALLREDUCE") == "mc":
+        ap.error("--global-batch cannot be used with AITJ_ALLREDUCE=mc: the multicast gradient path has no micro-batch "
+                 "accumulation")
     if args.doc_mask and not args.data:
         ap.error("--doc-mask needs --data")
     if args.data and args.model not in ("gpt2", "gpt2-tiny"):
