@@ -20,6 +20,7 @@ ANN_WORKER_RESCALE = "aitj.b200/rescale-trace"
 metrics.describe("aitj_rescale_seconds", "membership change observed by the workers -> first step at the new world "
                                          "(kind=rescale|recovery)")
 metrics.describe("aitj_job_samples_per_second", "whole-job training throughput reported by rank 0")
+metrics.describe("aitj_job_eval_loss", "mean held-out loss per token of the job's last evaluation, reported by rank 0")
 metrics.describe("aitj_job_recoveries_total", "in-place recoveries of faultTolerant jobs (a rank was lost, the others kept "
                                               "their state)")
 
@@ -43,9 +44,13 @@ def observe_worker_reports(old: dict, cur: dict) -> None:
     raw = a_cur.get(ANN_WORKER_METRICS)
     if raw and raw != a_old.get(ANN_WORKER_METRICS):
         try:
-            v = json.loads(raw).get("samples_per_sec")
+            rec = json.loads(raw)
+            v = rec.get("samples_per_sec")
             if v is not None:
                 metrics.set_gauge("aitj_job_samples_per_second", float(v), labels=labels)
+            v = rec.get("eval_loss")
+            if v is not None:
+                metrics.set_gauge("aitj_job_eval_loss", float(v), labels=labels)
         except (ValueError, TypeError, AttributeError):
             pass
 

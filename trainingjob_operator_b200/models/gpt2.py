@@ -90,6 +90,9 @@ class GPT2Engine(TransformerEngine):
         self.lnf_rstd = torch.empty(M, **f32)
         self.d_res = [torch.empty(M, C, **bf) for _ in range(2)]
         self.d_ln = torch.empty(M, C, **bf)
+        # evaluation (eval_forward): fp64 (sum of NLL, tokens); the cross-entropy partials are allocated on first use
+        self.eval_acc = torch.zeros(2, device=self.dev, dtype=torch.float64)
+        self._xent_part = self._xent_tgt = None
 
     def input_tensors(self) -> List[torch.Tensor]:
         """Device tensors a step reads its inputs from, in the order the data source yields them."""
@@ -101,6 +104,37 @@ class GPT2Engine(TransformerEngine):
     @torch.no_grad()
     def forward(self) -> torch.Tensor:
         """Consumes self.tok / self.tgt; fills self.loss (mean NLL) and leaves dlogits in self.logits."""
+        self._trunk()
+        self._linear(self.lnf, self.params.w16("wte"), self.logits)
+        return self._loss(self.M)
+
+    @torch.no_grad()
+    def eval_forward(self) -> torch.Tensor:
+        """Evaluation forward on self.tok / self.tgt (target -1: a padding row): the layers of ``forward``, then the logits
+        GEMM with the cross-entropy in its epilogue, so the logits never reach memory.  Fills self.losses with the
+        per-token NLL (0 for padding) and adds (sum of the NLL, tokens with a target) to the fp64 ``self.eval_acc``, which
+        the caller zeroes.  Leaves the logits, gradients and optimizer state as they are."""
+        if self.backend != "wgmma":
+            raise ValueError(f"evaluation needs the wgmma GEMM backend (its fused cross-entropy epilogue), not "
+                             f"{self.backend!r}")
+        F, P, cfg = self.F, self.params, self.cfg
+        if self._xent_part is None:
+            self._xent_part = torch.empty(self.M, F.xent_blocks(cfg.padded_vocab), 2, device=self.dev,
+                                          dtype=torch.float32)
+            self._xent_tgt = torch.empty(self.M, device=self.dev, dtype=torch.float32)
+        # a training step captured in a CUDA graph owns the tensors the attention forward leaves behind: keep them
+        kept = [(lb.att_in, lb.sdpa_ctx) for lb in self.layers]
+        self._trunk()
+        for lb, (att_in, ctx) in zip(self.layers, kept):
+            lb.att_in, lb.sdpa_ctx = att_in, ctx
+        wte = P.w16("wte")
+        F.gemm_xent(self.lnf, wte, self.tgt, cfg.vocab_size, self._xent_part, self._xent_tgt,
+                    block_n=self._bn(self.M, wte.shape[0], f"fwd:{wte.shape[0]}x{wte.shape[1]}"))
+        F.xent_finish(self._xent_part, self._xent_tgt, self.tgt, self.losses, self.eval_acc)
+        return self.eval_acc
+
+    def _trunk(self) -> None:
+        """Embeddings, the layers and the final LayerNorm: self.lnf from self.tok."""
         F, P = self.F, self.params
         F.embedding_fwd(self.tok, P.w16("wte"), P.w16("wpe"), self.x0, self.T)
         x = self.x0
@@ -115,8 +149,6 @@ class GPT2Engine(TransformerEngine):
             self._linear(lb.fc_act, P.w16(p + "fc2_w"), lb.res2, bias=P.w16(p + "fc2_b"), residual=lb.res1)
             x = lb.res2
         F.layernorm_fwd(x, P.w16("lnf_w"), P.w16("lnf_b"), self.lnf, self.lnf_mean, self.lnf_rstd)
-        self._linear(self.lnf, P.w16("wte"), self.logits)
-        return self._loss(self.M)
 
     @torch.no_grad()
     def _bwd_head(self) -> None:

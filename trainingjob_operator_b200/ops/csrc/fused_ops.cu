@@ -361,6 +361,60 @@ __global__ void __launch_bounds__(512, 2) softmax_xent_kernel(__nv_bfloat16* __r
   }
 }
 
+// ------------------------------------------------------------------ cross-entropy from the GEMM's partials (evaluation)
+// One warp per row: merge the row's (max, sum of exp) pairs of the EPI_XENT GEMM into its log-sum-exp, loss[row] =
+// lse - tgt_logit[row] (0 for a negative target).  acc[0] += the block's sum of losses, acc[1] += its rows with a target,
+// in fp64 with one atomic each per block, so micro-batches accumulate on the device without a host synchronisation.
+constexpr int kXentWarps = 8;
+
+__device__ __forceinline__ void lse_merge(float& m, float& s, float m2, float s2) {
+  if (s2 == 0.f) return;                       // (-inf, 0): a block wholly past the vocabulary
+  if (s == 0.f) { m = m2; s = s2; return; }
+  const float mn = fmaxf(m, m2);
+  s = s * __expf(m - mn) + s2 * __expf(m2 - mn);
+  m = mn;
+}
+
+__global__ void __launch_bounds__(kXentWarps * 32) xent_finish_kernel(const float2* __restrict__ part,
+                                                                      const float* __restrict__ tgt_logit,
+                                                                      const int64_t* __restrict__ target,
+                                                                      float* __restrict__ loss, double* __restrict__ acc,
+                                                                      int M, int nblk) {
+  __shared__ double red[kXentWarps][2];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  double wsum = 0.0, wcount = 0.0;              // lane 0's running totals of this warp's rows
+  for (int row = blockIdx.x * kXentWarps + warp; row < M; row += gridDim.x * kXentWarps) {
+    if (target[row] < 0) {
+      if (lane == 0) loss[row] = 0.f;
+      continue;
+    }
+    float m = -INFINITY, s = 0.f;
+    for (int b = lane; b < nblk; b += 32) {
+      const float2 p = part[static_cast<size_t>(row) * nblk + b];
+      lse_merge(m, s, p.x, p.y);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      const float m2 = __shfl_xor_sync(0xffffffffu, m, o), s2 = __shfl_xor_sync(0xffffffffu, s, o);
+      lse_merge(m, s, m2, s2);
+    }
+    if (lane == 0) {
+      const float l = m + logf(s) - tgt_logit[row];
+      loss[row] = l;
+      wsum += l;
+      wcount += 1.0;
+    }
+  }
+  if (lane == 0) { red[warp][0] = wsum; red[warp][1] = wcount; }
+  __syncthreads();
+  if (threadIdx.x < 2) {
+    double t = 0.0;
+#pragma unroll
+    for (int w = 0; w < kXentWarps; ++w) t += red[w][threadIdx.x];
+    if (t != 0.0) atomicAdd(acc + threadIdx.x, t);
+  }
+}
+
 // ------------------------------------------------------------------ bias grad: db[N] += colsum(dy[M,N])
 __global__ void __launch_bounds__(256) colsum_kernel(const __nv_bfloat16* __restrict__ dy, float* __restrict__ db,
                                                      int M, int N, int rows_per_block, int mc) {
@@ -734,6 +788,18 @@ int aitj_softmax_xent(void* logits, const void* target, void* loss, int M, int V
   }
   softmax_xent_kernel<<<M, 512, smem, S(stream)>>>(BF(logits), reinterpret_cast<const int64_t*>(target),
                                                     reinterpret_cast<float*>(loss), V, Vp, gscale);
+  return LAUNCH_OK();
+}
+
+// Finish the EPI_XENT GEMM's cross-entropy (see xent_finish_kernel): part float2 [M, nblk], tgt_logit fp32 [M], target
+// int64 [M] -> loss fp32 [M]; acc fp64 [2] += (sum of losses, rows with a target).
+int aitj_xent_finish(const void* part, const void* tgt_logit, const void* target, void* loss, void* acc, int M, int nblk,
+                     void* stream) {
+  if (M <= 0) return 0;
+  if (nblk < 1) return -1;
+  xent_finish_kernel<<<grid_for(M, kXentWarps, sms() * 8), kXentWarps * 32, 0, S(stream)>>>(
+      reinterpret_cast<const float2*>(part), reinterpret_cast<const float*>(tgt_logit),
+      reinterpret_cast<const int64_t*>(target), reinterpret_cast<float*>(loss), reinterpret_cast<double*>(acc), M, nblk);
   return LAUNCH_OK();
 }
 

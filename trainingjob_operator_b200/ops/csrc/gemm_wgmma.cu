@@ -43,6 +43,7 @@ enum : int {
   EPI_ACCUM = 64,     // out is fp32, red.global.add (split-K / grad accumulation)
   EPI_MC = 128,       // with EPI_ACCUM: `out` is an NVSwitch multicast address; reduce with multimem.red (GEMM + all-reduce in one kernel)
   EPI_COLSUM = 256,   // bf16 out only: colsum[N] += column sums of the stored output (set by aitj_gemm_set_colsum)
+  EPI_XENT = 512,     // no [M, N] output: per-row cross-entropy partials of the logits (set by aitj_gemm_set_xent)
   EPI_PEER = 16384    // with EPI_ACCUM: `out` lies in the symmetric, owner-sharded gradient buffer; every element is added into the
                       // copy of the rank that owns it (red.global.add over NVLink peer memory): weight-gradient GEMM +
                       // reduce-scatter in one kernel.  With split-K the splits add into the local copy and
@@ -62,6 +63,13 @@ struct GemmArgs {
   // EPI_COLSUM: colsum[N] += column sums of the stored output, i.e. the bias gradient of the layer whose input gradient
   // this GEMM produces
   float* colsum;
+  // EPI_XENT: for row r and 128-column block b, xent_part[r * xent_ld + b] <- (max, sum of exp(x - max)) over the
+  // block's columns below xent_vocab; xent_tgt[r] <- the logit of column xent_target[r].  Rows with a negative target
+  // are skipped.
+  const int64_t* xent_target;
+  float2* xent_part;
+  float* xent_tgt;
+  int xent_vocab, xent_ld;
 };
 
 struct WorkItem {
@@ -121,6 +129,61 @@ __device__ __forceinline__ void epilogue_f32(const GemmArgs& a, float (&acc)[kBN
       } else {
         red_add_v2_f32((flags & EPI_PEER) ? peer_ptr(p) : p, x0, x1);
       }
+    }
+  }
+}
+
+// Cross-entropy epilogue of one consumer warpgroup (EPI_XENT): the logits never leave the registers.  Each thread holds
+// two rows (r_base, r_base + 8) x kBN / 4 columns in the layout of epilogue_f32; the four lanes of a quad share a row,
+// so a row's (max, sum of exp) over a 128-column block is the quad's combination of its lanes' 32 values.  Lane 0 of
+// the quad stores the pair with one plain 8-byte store, and the lane holding the target column stores its logit: no
+// atomics, and each (row, block) and each row's target logit is written by exactly one thread.
+template <int kBN>
+__device__ __forceinline__ void epilogue_xent(const GemmArgs& a, const float (&acc)[kBN / 2], int r_base, int c_base,
+                                              int n0) {
+  constexpr float kLog2e = 1.4426950408889634f;
+  constexpr int kBlocks = kBN / 128;
+  const bool leader = (threadIdx.x & 3) == 0;
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int row = r_base + 8 * h;
+    // a padding row (negative target) or a row past M stores nothing; its quad still joins the shuffles, which take
+    // the whole warp
+    const long long tgt = row < a.M ? a.xent_target[row] : -1;
+    const bool live = tgt >= 0;
+#pragma unroll
+    for (int b = 0; b < kBlocks; ++b) {
+      const int blk_col0 = n0 + 128 * b;
+      if (blk_col0 >= a.N) break;
+      float mx = -INFINITY;
+#pragma unroll
+      for (int j = 16 * b; j < 16 * b + 16; ++j)
+#pragma unroll
+        for (int e = 0; e < 2; ++e)
+          if (c_base + 8 * j + e < a.xent_vocab) mx = fmaxf(mx, acc[4 * j + 2 * h + e]);
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+      // a block wholly past the vocabulary keeps (-inf, 0); the finish kernel skips such pairs
+      const float moff = mx == -INFINITY ? 0.f : mx * kLog2e;
+      float sum = 0.f;
+#pragma unroll
+      for (int j = 16 * b; j < 16 * b + 16; ++j)
+#pragma unroll
+        for (int e = 0; e < 2; ++e)
+          if (c_base + 8 * j + e < a.xent_vocab) sum += exp2f(fmaf(acc[4 * j + 2 * h + e], kLog2e, -moff));
+      sum += __shfl_xor_sync(0xffffffffu, sum, 1);
+      sum += __shfl_xor_sync(0xffffffffu, sum, 2);
+      if (live && leader) a.xent_part[static_cast<size_t>(row) * a.xent_ld + (blk_col0 >> 7)] = make_float2(mx, sum);
+    }
+    // the target column: register 4j + 2h + e of the lane whose quad offset covers it
+    const long long off = tgt - c_base;
+    if (live && off >= 0 && off < kBN && (off & 7) < 2) {
+      const int jt = static_cast<int>(off >> 3), et = static_cast<int>(off & 1);
+      float x = 0.f;
+#pragma unroll
+      for (int j = 0; j < kBN / 8; ++j)
+        if (j == jt) x = et ? acc[4 * j + 2 * h + 1] : acc[4 * j + 2 * h];
+      a.xent_tgt[row] = x;
     }
   }
 }
@@ -280,6 +343,7 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
   static_assert(!kBMN || kSliceN % 64 == 0, "MN-major B slices are whole 64-column chunks");
   static_assert(!(kEpi & EPI_RESIDUAL) || !(kEpi & (EPI_DGELU | EPI_SAVE_PRE)), "one second bf16 tensor per epilogue");
   static_assert(!(kEpi & EPI_DGELU) || !(kEpi & EPI_SAVE_PRE), "one second bf16 tensor per epilogue");
+  static_assert(!(kEpi & EPI_XENT) || kEpi == (EPI_XENT | EPI_OUT_F32), "the cross-entropy epilogue combines with no other");
   constexpr int kStaging = bf16_out<kEpi>() ? kStagingBytes : 0;
   const CUtensorMap* in_map = (kEpi & EPI_RESIDUAL) ? &tmap_res : &tmap_aux;
 
@@ -416,6 +480,8 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
       if (nk > 0) {
         if constexpr (bf16_out<kEpi>()) {
           if (m0 < args.M) epilogue_bf16<kBN, kEpi>(args, &tmap_out, &tmap_aux, in_map, acc, st, m0, n0);
+        } else if constexpr ((kEpi & EPI_XENT) != 0) {
+          epilogue_xent<kBN>(args, acc, m0 + (warp & 3) * 16 + (lane >> 2), n0 + 2 * (lane & 3), n0);
         } else {
           epilogue_f32<kBN, kEpi>(args, acc, m0 + (warp & 3) * 16 + (lane >> 2), n0 + 2 * (lane & 3));
         }
@@ -560,6 +626,9 @@ static const GemmKernel kGemmKernels[] = {
     GEMM_TILES(false, false, EPI_BIAS),
     GEMM_TILES(false, false, EPI_BIAS | EPI_GELU | EPI_SAVE_PRE),
     GEMM_TILES(false, false, EPI_BIAS | EPI_RESIDUAL),
+    // evaluation: the logits GEMM with the cross-entropy epilogue (GPT2Engine.eval_forward); its only outputs are fp32
+    // plain stores (the partials), so its kernel is keyed as an fp32 variant: no staging slots, no TMA store
+    GEMM_TILES(false, false, EPI_XENT | EPI_OUT_F32),
     // epilogues of the other layouts, checked on this one (selfcheck)
     GEMM_TILES(false, false, EPI_DGELU),
     GEMM_TILES(false, false, EPI_DGELU | EPI_COLSUM),
@@ -582,6 +651,12 @@ static const GemmKernel kGemmKernels[] = {
 }  // namespace aitj
 
 static float* g_gemm_colsum = nullptr;   // consumed by the next aitj_gemm_bf16 call
+static struct {
+  const int64_t* target;
+  float2* part;
+  float* tgt;
+  int vocab;
+} g_gemm_xent = {nullptr, nullptr, nullptr, 0};   // consumed by the next aitj_gemm_bf16 call
 
 extern "C" {
 
@@ -589,14 +664,37 @@ extern "C" {
 // One-shot: cleared by that call.
 int aitj_gemm_set_colsum(void* buf) { g_gemm_colsum = reinterpret_cast<float*>(buf); return 0; }
 
+// The next aitj_gemm_bf16 call with flags == EPI_XENT writes no output: for every row r with target[r] >= 0 (int64) it
+// stores part[r, b] = (max, sum of exp(x - max)) (float2 [M, ceil(N / 128)]) over the columns c < vocab of each
+// 128-column block b of row r of the product, and tgt_logit[r] (fp32) = its column target[r].  One-shot: cleared by
+// that call.  aitj_xent_finish (fused_ops.cu) turns the partials into per-row losses.
+int aitj_gemm_set_xent(const void* target, void* part, void* tgt_logit, int vocab) {
+  g_gemm_xent.target = reinterpret_cast<const int64_t*>(target);
+  g_gemm_xent.part = reinterpret_cast<float2*>(part);
+  g_gemm_xent.tgt = reinterpret_cast<float*>(tgt_logit);
+  g_gemm_xent.vocab = vocab;
+  return 0;
+}
+
 // Returns 0 on success. See file header for operand conventions. lda/ldb/ldc in elements.
 // block_n: 128 or 256 (0 = auto); 512 / 1024: 128x256 tiles in clusters of 2 / 4 CTAs sharing B by TMA multicast.
 // split_k > 1 requires EPI_ACCUM. max_ctas: 0 = all SMs.  -7: no kernel is compiled for this operand layout and
-// epilogue (kGemmKernels).
+// epilogue (kGemmKernels).  EPI_XENT (after aitj_gemm_set_xent) takes no other bit and no split, and `out` may be null;
+// -8: it was asked for without its buffers, with another bit or a split, or with vocab outside [1, N].
 int aitj_gemm_bf16(const void* A, const void* B, void* out, int M, int N, int K, int lda, int ldb, int ldc,
                    int a_mn, int b_mn, const void* bias, const void* residual, void* aux, int flags, int split_k,
                    int block_n, int max_ctas, void* stream_ptr) {
   using namespace aitj;
+  const auto xent = g_gemm_xent;
+  g_gemm_xent = {nullptr, nullptr, nullptr, 0};
+  if (flags & EPI_XENT) {
+    // the max and the sum of exponentials of a row cannot be formed from the partial products of a K split
+    if (flags != EPI_XENT || split_k > 1 || !xent.target || !xent.part || !xent.tgt || xent.vocab < 1 ||
+        xent.vocab > N || (reinterpret_cast<uintptr_t>(xent.part) & 7))
+      return -8;
+  } else if (xent.target) {
+    return -8;                                   // cross-entropy buffers given to a GEMM without EPI_XENT
+  }
   if (M <= 0 || N <= 0 || K <= 0) return 0;
   if ((N & 7) || (ldc & 7) || (lda & 7) || (ldb & 7)) return -1;
   // TMA needs 16-byte aligned tensors
@@ -619,7 +717,12 @@ int aitj_gemm_bf16(const void* A, const void* B, void* out, int M, int N, int K,
   args.aux = reinterpret_cast<__nv_bfloat16*>(aux);
   args.colsum = g_gemm_colsum;
   g_gemm_colsum = nullptr;
-  if (args.colsum && (flags & (EPI_OUT_F32 | EPI_ACCUM))) return -6;   // column sums of a bf16 output only
+  if (args.colsum && (flags & (EPI_OUT_F32 | EPI_ACCUM | EPI_XENT))) return -6;   // column sums of a bf16 output only
+  args.xent_target = xent.target;
+  args.xent_part = xent.part;
+  args.xent_tgt = xent.tgt;
+  args.xent_vocab = xent.vocab;
+  args.xent_ld = (N + 127) / 128;
   args.tiles_m = (M + BLOCK_M - 1) / BLOCK_M;
   args.tiles_n = (N + block_n - 1) / block_n;
   args.k_blocks = (K + BLOCK_K - 1) / BLOCK_K;
@@ -630,6 +733,7 @@ int aitj_gemm_bf16(const void* A, const void* B, void* out, int M, int N, int K,
   const bool peer_move = (flags & EPI_PEER) && args.split_k > 1;
   int epi = flags & ~EPI_COLSUM;
   if (args.colsum) epi |= EPI_COLSUM;
+  if (flags & EPI_XENT) epi |= EPI_OUT_F32;
   if (peer_move) epi &= ~EPI_PEER;
   const GemmKernel* kernel = nullptr;
   for (const GemmKernel& k : kGemmKernels)
@@ -645,7 +749,7 @@ int aitj_gemm_bf16(const void* A, const void* B, void* out, int M, int N, int K,
   if (!b_mn) rc = encode_2d(&maps.b, B, K, N, ldb, BLOCK_K, block_n / cm);
   else       rc = encode_2d(&maps.b, B, N, K, ldb, 64, BLOCK_K);
   if (rc) return rc - 1000;
-  if (!(flags & (EPI_OUT_F32 | EPI_ACCUM))) {
+  if (!(flags & (EPI_OUT_F32 | EPI_ACCUM | EPI_XENT))) {
     rc = encode_2d(&maps.out, out, N, M, ldc, 64, 64);
     if (!rc && (flags & (EPI_SAVE_PRE | EPI_DGELU))) rc = encode_2d(&maps.aux, aux, N, M, ldc, 64, 64);
     if (!rc && (flags & EPI_RESIDUAL)) rc = encode_2d(&maps.res, residual, N, M, ldc, 64, 64);

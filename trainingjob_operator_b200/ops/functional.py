@@ -20,6 +20,7 @@ EPI_ACCUM = 64
 EPI_MC = 128
 EPI_PEER = 16384
 EPI_COLSUM = 256   # set by the library when a colsum buffer is given
+EPI_XENT = 512     # gemm_xent: per-row cross-entropy partials instead of an output (kernel keyed EPI_XENT | EPI_OUT_F32)
 
 # aitj_gemm_bf16: out, aux or residual is not 16-byte aligned (the epilogue reaches them by TMA)
 GEMM_MISALIGNED = -4
@@ -138,9 +139,43 @@ def gemm(a, b, out, *, a_mn=False, b_mn=False, bias=None, residual=None, aux=Non
 def epilogue_name(flags: int) -> str:
     names = [n for n, bit in (("BIAS", EPI_BIAS), ("GELU", EPI_GELU), ("RESIDUAL", EPI_RESIDUAL),
                               ("SAVE_PRE", EPI_SAVE_PRE), ("DGELU", EPI_DGELU), ("OUT_F32", EPI_OUT_F32),
-                              ("ACCUM", EPI_ACCUM), ("MC", EPI_MC), ("PEER", EPI_PEER), ("COLSUM", EPI_COLSUM))
+                              ("ACCUM", EPI_ACCUM), ("MC", EPI_MC), ("PEER", EPI_PEER), ("COLSUM", EPI_COLSUM),
+                              ("XENT", EPI_XENT))
              if flags & bit]
     return "|".join(names) or "none"
+
+
+def xent_blocks(n: int) -> int:
+    """Column blocks of ``gemm_xent``'s partials for a product with ``n`` columns."""
+    return (n + 127) // 128
+
+
+def gemm_xent(x, w, target, vocab, part, tgt_logit, block_n=0):
+    """Cross-entropy partials of the logits x[M,K] @ w[N,K]^T, which are never written out: for every row r with
+    target[r] >= 0 (int64 [M]), part[r, b] <- (max, sum of exp(z - max)) over the columns z < ``vocab`` of 128-column
+    block b (fp32 [M, xent_blocks(N), 2]) and tgt_logit[r] <- the logit of column target[r] (fp32 [M]), from the fp32
+    accumulators.  ``xent_finish`` turns them into per-row losses.  ``block_n`` as for ``gemm``."""
+    assert x.dtype == torch.bfloat16 and w.dtype == torch.bfloat16 and x.dim() == 2 and w.dim() == 2
+    assert x.stride(1) == 1 and w.stride(1) == 1
+    M, K = x.shape
+    N, Kw = w.shape
+    assert K == Kw, (x.shape, w.shape)
+    assert 0 < vocab <= N, (vocab, N)
+    assert target.dtype == torch.int64 and target.numel() == M and target.is_contiguous()
+    assert part.dtype == torch.float32 and tuple(part.shape) == (M, xent_blocks(N), 2) and part.is_contiguous()
+    assert tgt_logit.dtype == torch.float32 and tgt_logit.numel() == M
+    lib.load().aitj_gemm_set_xent(target.data_ptr(), part.data_ptr(), tgt_logit.data_ptr(), int(vocab))
+    lib.call("aitj_gemm_bf16", x.data_ptr(), w.data_ptr(), None, M, N, K, x.stride(0), w.stride(0), 0, 0, 0, None,
+             None, None, EPI_XENT, 1, int(block_n), 0, _stream())
+
+
+def xent_finish(part, tgt_logit, target, loss, acc):
+    """loss[r] <- log-sum-exp of row r's ``gemm_xent`` partials - tgt_logit[r] (0 where target[r] < 0); acc (fp64 [2])
+    += (sum of the losses, rows with a target)."""
+    M, nblk = part.shape[0], part.shape[1]
+    assert acc.dtype == torch.float64 and acc.numel() == 2 and loss.dtype == torch.float32 and loss.numel() == M
+    lib.call("aitj_xent_finish", part.data_ptr(), tgt_logit.data_ptr(), target.data_ptr(), loss.data_ptr(),
+             acc.data_ptr(), M, nblk, _stream())
 
 
 def gemm_epilogue(out, *, bias=None, residual=None, aux=None, gelu=False, dgelu=False, save_pre=False,

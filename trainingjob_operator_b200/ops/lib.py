@@ -66,6 +66,8 @@ _SIGS = {
     "aitj_attn_fwd": [_P, _P, _P, _P, _I, _I, _I, _I, _F, _P],
     "aitj_attn_bwd": [_P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _F, _P],
     "aitj_gemm_set_colsum": [_P],
+    "aitj_gemm_set_xent": [_P, _P, _P, _I],
+    "aitj_xent_finish": [_P, _P, _P, _P, _P, _I, _I, _P],
     "aitj_layernorm_fwd": [_P, _P, _P, _P, _P, _P, _I, _I, _F, _P],
     "aitj_layernorm_bwd": [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _P],
     "aitj_embedding_fwd": [_P, _P, _P, _P, _I, _I, _I, _P],
@@ -139,7 +141,7 @@ def _label(name: str, args) -> str:
         return name[5:]
     a_mn, b_mn, flags, split_k, block_n = args[9], args[10], args[14], args[15], args[16]
     kind = "wgrad" if a_mn and b_mn else ("dgrad" if b_mn else "fwd")
-    extra = "+peer" if flags & 16384 else ("+mc" if flags & 128 else "")
+    extra = "+peer" if flags & 16384 else ("+mc" if flags & 128 else ("+xent" if flags & 512 else ""))
     return f"gemm:{kind}{extra} N={args[4]} K={args[5]} bn={block_n} sk={split_k}"
 
 

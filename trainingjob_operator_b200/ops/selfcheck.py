@@ -845,6 +845,106 @@ def case_gpt2_docs():
     return ok
 
 
+def _xent_ref(a, w, target, V):
+    """fp64 per-row NLL of the logits a @ w^T over the first V columns (0 for a negative target)."""
+    z = (a.double() @ w.double().t())[:, :V]
+    lse = torch.logsumexp(z, 1)
+    t = target.clamp(min=0)
+    nll = lse - z.gather(1, t[:, None])[:, 0]
+    return torch.where(target >= 0, nll, torch.zeros_like(nll))
+
+
+def case_gemm_xent():
+    """The cross-entropy epilogue (gemm_xent + xent_finish) in every tile configuration against an fp64 log-softmax of
+    the same bf16 operands: M not a multiple of 128, V < N with N not a multiple of 256, targets in the last partial
+    tile, padding rows (target -1), logits of standard deviation ~30 so that the max shift matters."""
+    ok = True
+    g = torch.Generator(device="cuda").manual_seed(11)
+    for M, N, V, K in ((1000, 1000, 937, 768), (4133, 50304, 50257, 768)):
+        a = torch.randn(M, K, device="cuda", generator=g).bfloat16()
+        w = (torch.randn(N, K, device="cuda", generator=g) * (30.0 / K ** 0.5)).bfloat16()
+        target = torch.randint(0, V, (M,), device="cuda", generator=g)
+        target[::7] = -1
+        target[1::5] = V - 1 - torch.randint(0, min(V, 200) // 2, (len(target[1::5]),), device="cuda", generator=g)
+        ref = _xent_ref(a, w, target, V)
+        for bn in (128, 256, 512, 1024):
+            part = torch.full((M, F.xent_blocks(N), 2), float("nan"), device="cuda")
+            tgt_logit = torch.empty(M, device="cuda")
+            loss = torch.full((M,), float("nan"), device="cuda")
+            acc = torch.zeros(2, device="cuda", dtype=torch.float64)
+            F.gemm_xent(a, w, target, V, part, tgt_logit, block_n=bn)
+            F.xent_finish(part, tgt_logit, target, loss, acc)
+            F.xent_finish(part, tgt_logit, target, loss, acc)      # accumulates
+            torch.cuda.synchronize()
+            err = float((loss.double() - ref).abs().max())
+            rows = int((target >= 0).sum())
+            sum_err = abs(float(acc[0]) / 2 - float(ref.sum())) / float(ref.sum())
+            good = err <= 1e-3 and float(acc[1]) == 2 * rows and sum_err < 1e-6 and bool(torch.isfinite(loss).all())
+            good &= bool((loss[target < 0] == 0).all())
+            print(f"  gemm_xent M={M} N={N} V={V} K={K} block_n={bn}: max |loss - fp64| {err:.2e} (tol 1e-3), rows "
+                  f"{float(acc[1]) / 2:.0f} of {rows}, sum rel err {sum_err:.1e} {'ok' if good else 'FAIL'}", flush=True)
+            ok &= good
+    # refused: another epilogue bit, or a split
+    for bad in (dict(flags=F.EPI_XENT | F.EPI_BIAS), dict(split_k=2)):
+        part = torch.empty(64, 1, 2, device="cuda")
+        x = torch.zeros(64, 128, device="cuda", dtype=torch.bfloat16)
+        w = torch.zeros(128, 128, device="cuda", dtype=torch.bfloat16)
+        tgt = torch.zeros(64, device="cuda", dtype=torch.int64)
+        t = torch.empty(64, device="cuda")
+        F.lib.load().aitj_gemm_set_xent(tgt.data_ptr(), part.data_ptr(), t.data_ptr(), 128)
+        rc = F.lib.load().aitj_gemm_bf16(x.data_ptr(), w.data_ptr(), None, 64, 128, 128, 128, 128, 0, 0, 0, None, None,
+                                         None, bad.get("flags", F.EPI_XENT), bad.get("split_k", 1), 0, 0,
+                                         torch.cuda.current_stream().cuda_stream)
+        print(f"  gemm_xent refuses {bad}: code {rc}")
+        ok &= rc == -8
+    return ok
+
+
+def case_gpt2_eval():
+    """GPT2Engine.eval_forward at GPT-2 small, B16 x T1024, with and without a document mask: the mean NLL equals the
+    training forward's (which rounds the logits to bf16) within 2e-3 and the fp32 reference's within 5e-3 relative,
+    and parameters, gradients, optimizer state and the logits buffer are left bit-identical."""
+    from ..models.gpt2 import GPT2Config, GPT2Engine, GPT2Reference
+
+    ok = True
+    cfg = GPT2Config.small()
+    B, T = 16, 1024
+    for doc_mask in (False, True):
+        eng = GPT2Engine(cfg, B, T, "cuda", seed=3, doc_mask=doc_mask)
+        if doc_mask:
+            tok, ds = _doc_tokens(B, T, cfg.vocab_size, 50256, [[300, 1, 200, 523], [1024], [7, 640, 377]], 5)
+            ins = (tok.cuda(), torch.roll(tok, -1, dims=1).cuda(), ds.cuda())
+        else:
+            tok = torch.randint(0, cfg.vocab_size, (B, T), generator=torch.Generator().manual_seed(5))
+            ins = (tok.cuda(), torch.roll(tok, -1, dims=1).cuda())
+        for dst, src in zip(eng.input_tensors(), ins):
+            dst.copy_(src.reshape(-1))
+        eng.params.g32.normal_()
+        eng.params.m.normal_()
+        before = [t.clone() for t in eng.params.state_tensors()] + [eng.params.g32.clone(), eng.params.p16.clone()]
+        eng.forward()
+        logits = eng.logits.clone()
+        train = float(eng.loss.item())
+        eng.eval_acc.zero_()
+        eng.eval_forward()
+        torch.cuda.synchronize()
+        ev = float(eng.eval_acc[0] / eng.eval_acc[1])
+        after = [t for t in eng.params.state_tensors()] + [eng.params.g32, eng.params.p16]
+        same = all(torch.equal(x, y) for x, y in zip(before, after)) and torch.equal(logits, eng.logits)
+        with torch.no_grad():
+            ref = GPT2Reference(cfg, eng.params).cuda()
+            rl = float(ref(*ins[:2], ins[2] if doc_mask else None))
+        del ref
+        good = abs(ev - train) <= 2e-3 and abs(ev - rl) <= 5e-3 * abs(rl) and float(eng.eval_acc[1]) == B * T and same
+        print(f"  gpt2_eval doc_mask={doc_mask}: eval {ev:.6f} forward {train:.6f} (|d| {abs(ev - train):.1e}, tol 2e-3) "
+              f"fp32 reference {rl:.6f} (rel {abs(ev - rl) / abs(rl):.1e}, tol 5e-3), state untouched {same} "
+              f"{'ok' if good else 'FAIL'}", flush=True)
+        ok &= good
+        del eng
+        torch.cuda.empty_cache()
+    return ok
+
+
 def case_gemm_cluster():
     """Cluster kernels (block_n=512 / 1024), whose consumers hand each ring stage back to every CTA of the cluster: a
     single work item, work items spread unevenly over the clusters, split-K whose last split is shorter, M, N and K tails, and
@@ -1009,6 +1109,8 @@ def case_accumulation():
 
 
 CASES = {
+    "gemm_xent": case_gemm_xent,
+    "gpt2_eval": case_gpt2_eval,
     "accumulation": case_accumulation,
     "gemm_cluster": case_gemm_cluster,
     "attention": case_attention,

@@ -158,22 +158,25 @@ class TokenFileData:
             s["event"] = None
         return s
 
-    def stage(self, first: int, B: int) -> List[torch.Tensor]:
-        """Samples [first, first + B) -> pinned (tok, tgt[, doc_start]) of B*T elements each."""
+    def stage(self, first: int, B: int, count: Optional[int] = None) -> List[torch.Tensor]:
+        """Samples [first, first + B) -> pinned (tok, tgt[, doc_start]) of B*T elements each.  ``count`` < B: only
+        samples [first, first + count) are read, and the rows of the others carry token 0 and target -1 (no loss)."""
         T = self.T
-        toks = np.empty((B, T + 1), dtype=np.uint16)
-        for b in range(B):
+        count = B if count is None else count
+        toks = np.zeros((B, T + 1), dtype=np.uint16)
+        for b in range(count):
             toks[b] = self.window(first + b)         # validated before anything is staged
         s = self._slot(B)
         w = toks.astype(np.int64)
         s["tok"].numpy().reshape(B, T)[:] = w[:, :-1]
         s["tgt"].numpy().reshape(B, T)[:] = w[:, 1:]
+        s["tgt"].numpy().reshape(B, T)[count:] = -1
         out = [s["tok"], s["tgt"]]
         if self.doc_mask:
             s["doc"].numpy().reshape(B, T)[:] = doc_starts(w[:, :-1], self.eot)
             out.append(s["doc"])
         self._last = s
-        self.samples_read = list(range(first, first + B))
+        self.samples_read = list(range(first, first + count))
         return out
 
     def in_flight(self) -> None:

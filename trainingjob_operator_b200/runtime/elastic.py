@@ -189,6 +189,8 @@ class ElasticWatcher:
         keep = {k: result.get(k) for k in ("samples_per_sec", "ms_per_step", "global_batch", "world", "steps_done",
                                            "loss_first", "loss_last", "gpu_launches", "cuda_graph")}
         keep["recoveries"] = len(result.get("recoveries") or [])
+        if result.get("evals"):
+            keep.update(eval_loss=result["evals"][-1]["loss"], eval_step=result["evals"][-1]["step"])
         t = getattr(self, "_live_thread", None)
         if t is not None:
             t.join(5.0)                     # an interim report in flight must not land after (and over) the final one

@@ -12,7 +12,7 @@ from __future__ import annotations
 import math
 import os
 import time
-from typing import List, Optional
+from typing import List, Optional, Tuple
 
 import torch
 import torch.distributed as dist
@@ -403,6 +403,23 @@ class EngineTrainer:
         if self.cuda:
             torch.cuda.current_stream().synchronize()
         return float(self.loss_host[0])
+
+    # ------------------------------------------------------------------ evaluation
+    def evaluate(self, micro_inputs) -> Tuple[float, int]:
+        """Evaluation forwards (``engine.eval_forward``) of this rank's micro-batches, launched eagerly: ``micro_inputs``
+        yields each one's inputs in pinned host memory, as ``accumulate`` takes them.  The ranks' (sum of NLL, tokens)
+        are summed by one all-reduce on the job's group, which a rank without micro-batches joins too.  Returns the
+        job's (sum of NLL, tokens); touches no parameter, gradient or optimizer state."""
+        e = self.engine
+        e.eval_acc.zero_()
+        for host in micro_inputs:
+            for dst, src in zip(e.input_tensors(), host):
+                dst.copy_(src, non_blocking=True)
+            e.eval_forward()
+        if self.world > 1:
+            dist.all_reduce(e.eval_acc, group=self.group)
+        total = e.eval_acc.cpu()
+        return float(total[0]), int(total[1])
 
     def state_tensors(self) -> List[torch.Tensor]:
         return self.engine.params.state_tensors()

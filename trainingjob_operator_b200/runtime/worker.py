@@ -77,6 +77,16 @@ class EngineAdapter:
             else:
                 self.data = SyntheticTokens(cfg.vocab_size, batch, seq, n_batches=4, seed=args.seed + 1)
             self.flops_per_step = flops_per_token(cfg, seq) * batch * seq
+            if getattr(args, "eval_data", ""):
+                from .data import DataError, TokenFileData
+
+                # held-out windows [0, eval_samples) of their own stream: no position, so nothing to hand off or save
+                self.eval_data = TokenFileData(args.eval_data, seq, cfg.vocab_size, doc_mask=doc_mask,
+                                               eot=args.eot_token, pin=device != "cpu")
+                self.eval_samples = args.eval_samples or 20 * batch
+                if self.eval_samples > self.eval_data.n_windows:
+                    raise DataError(f"--eval-samples {self.eval_samples}: --eval-data {args.eval_data!r} holds only "
+                                    f"{self.eval_data.n_windows} windows of {seq + 1} tokens")
         self.cfg = cfg
         self.batch, self.seq = batch, seq
         self.h2d_bytes = self.data.bytes_per_sample * batch if hasattr(self, "data_position") else \
@@ -88,6 +98,8 @@ class EngineAdapter:
                          "gemm": args.gemm}
         if hasattr(self, "data_position"):
             self.describe.update(data=args.data, doc_mask=self.engine.doc_mask, windows=self.data.n_windows)
+        if hasattr(self, "eval_data"):
+            self.describe.update(eval_data=args.eval_data, eval_samples=self.eval_samples)
 
     def bind(self, group=None, warm_up: bool = False) -> None:
         """(Re-)build the trainer for the current process group; the micro-batch plan follows its world size.
@@ -136,6 +148,30 @@ class EngineAdapter:
             heartbeat()                    # a long accumulated step must not look like a hang to the agent
         self.samples_read = read
         self.data_position += plan.global_batch
+
+    def eval_plan(self):
+        """This rank's share of the evaluation: the held-out windows [0, S) cut into ceil(S / B) micro-batches, assigned
+        to the ranks as ``runtime.accumulation`` assigns a step's micro-batches."""
+        from .accumulation import micro_batch_plan
+
+        B = self.batch
+        k = -(-self.eval_samples // B)
+        return micro_batch_plan(k * B, B, self.trainer.world, self.trainer.rank)
+
+    def _eval_inputs(self, progress=None):
+        S = self.eval_samples
+        for first, count in self.eval_plan().windows(0):
+            yield self.eval_data.stage(first, count, min(count, S - first))   # past S: token 0, target -1
+            self.eval_data.in_flight()
+            heartbeat()
+            if progress is not None:
+                progress()
+
+    def evaluate(self, progress=None) -> Dict[str, Any]:
+        """The job's mean NLL per token over the held-out windows (collective: every rank calls it).  ``progress`` is
+        called after each of this rank's micro-batches is enqueued."""
+        total, tokens = self.trainer.evaluate(self._eval_inputs(progress))
+        return {"loss": total / max(1, tokens), "tokens": tokens, "samples": self.eval_samples}
 
     def discard_step(self) -> None:
         self.engine.params.g32.zero_()
@@ -552,7 +588,25 @@ def run(args) -> Dict[str, Any]:
     # rank 0 publishes its wall-clock throughput every AITJ_REPORT_EVERY seconds (0 = only the final, device-timed result)
     report_every = float(os.environ.get("AITJ_REPORT_EVERY", "10"))
     live_t0, live_step0 = time.time(), step
-    while step < total and not stop["flag"]:
+    # held-out evaluation (--eval-data): at the boundary before every step that is a multiple of --eval-every, and once
+    # after the last step.  A boundary's evaluation is done once it has completed.  Every (re-)bind to a new generation
+    # forgets that (last_eval_step = -1): a joiner knows nothing of it, so after a rescale or a recovery at a boundary
+    # that was already evaluated -- a peer lost in the step right after an evaluation -- every rank of the new generation
+    # evaluates it again, and all of them issue the same collectives.
+    evals: List[Dict[str, Any]] = []
+    last_eval_step = -1
+    # evaluation inside the timed region (device ms, wall ms, kernel launches), taken out of the step figures; and the
+    # evaluation wall time since the last interim report, taken out of its throughput
+    eval_ms_timed = eval_wall_timed = 0.0
+    eval_launches_timed = 0
+    live_eval_s = 0.0
+
+    def eval_due(s: int) -> bool:
+        if not hasattr(adapter, "eval_data") or s == last_eval_step:
+            return False
+        return (s > 0 and args.eval_every > 0 and s % args.eval_every == 0) or (args.steps > 0 and s >= total)
+
+    while (step < total or eval_due(step)) and not stop["flag"]:
         if breaker is not None:
             breaker.progress(generation)
             # patience from this generation's completed steps: the first step on a freshly bound trainer captures CUDA
@@ -586,6 +640,7 @@ def run(args) -> Dict[str, Any]:
                         generation, world, port = got["generation"], got["world"], got["port"]
                     t2 = time.time()
                     adapter.bind(None)
+                    last_eval_step = -1
                     step = guarded(breaker, generation, lambda: sync_state(adapter, step, device))
                     heartbeat(force=True)
                     watcher.adopted(generation, world)
@@ -607,6 +662,44 @@ def run(args) -> Dict[str, Any]:
                 t_epoch0 = time.time()
                 timed_from = step
                 launches0 = oplib.LAUNCHES
+            if eval_due(step):
+                if breaker is not None:
+                    breaker.progress(generation)
+                    breaker.in_step = True
+                t_eval = time.perf_counter()
+                launches_before = oplib.LAUNCHES
+                e0 = e1 = None
+                if use_cuda:
+                    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                    e0.record()
+                try:
+                    # an evaluation is as long as its micro-batches make it: the stall breaker sees progress after each
+                    # one, not the patience of a single training step for the whole of it
+                    rec = adapter.evaluate(progress=None if breaker is None else lambda: breaker.progress(generation))
+                finally:
+                    if breaker is not None:
+                        breaker.in_step = False
+                if breaker is not None and breaker.tripped:
+                    raise RuntimeError("the communicator was aborted while an evaluation was in flight")
+                wall_ms = (time.perf_counter() - t_eval) * 1e3
+                if use_cuda:
+                    e1.record()
+                    e1.synchronize()
+                ms = e0.elapsed_time(e1) if use_cuda else wall_ms
+                if timed_from >= 0:
+                    eval_ms_timed += ms
+                    eval_wall_timed += wall_ms
+                    eval_launches_timed += oplib.LAUNCHES - launches_before
+                live_eval_s += wall_ms / 1e3
+                rec = {"step": step, "loss": rec["loss"], "tokens": rec["tokens"], "samples": rec["samples"],
+                       "ms": round(ms, 3)}
+                evals.append(rec)
+                last_eval_step = step
+                if rank == 0:
+                    print(f"[worker {rank}] step {step}: eval loss {rec['loss']:.6f} over {rec['samples']} held-out "
+                          f"windows ({rec['tokens']} tokens) in {ms:.1f} ms", flush=True)
+                if step >= total:
+                    continue          # the evaluation after the last step: the loop ends here
             if breaker is not None:
                 breaker.progress(generation)
                 breaker.in_step = True
@@ -670,6 +763,7 @@ def run(args) -> Dict[str, Any]:
                 breaker.tripped = False
                 breaker.progress(generation)
             adapter.bind(None)
+            last_eval_step = -1
             # the hand-off is a chain of collectives on the new group: if ANOTHER peer dies under it, a still newer
             # generation is published and the breaker must be able to get this rank out of it
             try:
@@ -716,13 +810,15 @@ def run(args) -> Dict[str, Any]:
             if watcher is not None:
                 watcher.report_trace(rank, trace)
         if rank == 0 and watcher is not None and report_every > 0 and time.time() - live_t0 >= report_every:
-            dt, n = time.time() - live_t0, step - live_step0
-            if n > 0:
+            dt, n = time.time() - live_t0 - live_eval_s, step - live_step0
+            if n > 0 and dt > 0:
                 G = adapter.plan.global_batch
-                watcher.report_live(rank, {"samples_per_sec": round(G * n / dt, 2),
-                                           "ms_per_step": round(dt * 1e3 / n, 3), "world": world, "steps_done": step,
-                                           "global_batch": G, "recoveries": len(recoveries)})
-            live_t0, live_step0 = time.time(), step
+                live = {"samples_per_sec": round(G * n / dt, 2), "ms_per_step": round(dt * 1e3 / n, 3), "world": world,
+                        "steps_done": step, "global_batch": G, "recoveries": len(recoveries)}
+                if evals:
+                    live.update(eval_loss=evals[-1]["loss"], eval_step=evals[-1]["step"])
+                watcher.report_live(rank, live)
+            live_t0, live_step0, live_eval_s = time.time(), step, 0.0
         if args.ckpt_every > 0 and step % args.ckpt_every == 0:
             adapter.prepare_state()
             if rank == 0:
@@ -735,6 +831,8 @@ def run(args) -> Dict[str, Any]:
                               "recoveries": recoveries, "trace": trace}
     if hasattr(adapter, "data_position"):
         result["data_position"] = adapter.data_position
+    if hasattr(adapter, "eval_data"):
+        result.update(evals=evals, eval_loss_last=evals[-1]["loss"] if evals else None)
     if breaker is not None:
         breaker.stop()
     if _CKPT.get("writer") is not None:
@@ -747,15 +845,16 @@ def run(args) -> Dict[str, Any]:
         t_epoch1 = time.time()
         if world > 1:
             dist.barrier()
-        wall = time.perf_counter() - t_wall0
-        dev_ms = ev0.elapsed_time(ev1) if use_cuda else wall * 1e3
+        wall_total = time.perf_counter() - t_wall0
+        dev_ms = (ev0.elapsed_time(ev1) if use_cuda else wall_total * 1e3) - eval_ms_timed
+        wall = wall_total - eval_wall_timed / 1e3
         dev_ms = max_over_ranks(dev_ms, device)
         plan = adapter.plan
         global_batch = plan.global_batch
         result.update({"timed_steps": n_timed, "timed_from_step": timed_from,
                        "timed_region_epoch": [t_epoch0, t_epoch1]})
         graph_launches = adapter.launches_per_step()
-        eager_launches = (oplib.LAUNCHES - launches0)
+        eager_launches = oplib.LAUNCHES - launches0 - eval_launches_timed
         result.update({
             "ms_per_step": dev_ms / n_timed,
             "samples_per_sec": global_batch * n_timed / (dev_ms / 1e3),
@@ -825,7 +924,22 @@ def parse_args(argv=None):
     ap.add_argument("--global-batch", type=int, default=0, metavar="G",
                     help="samples per optimizer step for the whole job, at any world size: each step trains G / --batch "
                          "micro-batches, spread over the ranks, and sums their gradients (0 = world size x --batch)")
+    ap.add_argument("--eval-data", default="", metavar="PATH_OR_GLOB",
+                    help="evaluate on these held-out token shards (formats as --data; GPT-2 models, wgmma GEMMs)")
+    ap.add_argument("--eval-samples", type=int, default=0, metavar="S",
+                    help="held-out windows per evaluation, the first S of the stream (0 = 20 x --batch)")
+    ap.add_argument("--eval-every", type=int, default=0, metavar="N",
+                    help="evaluate before every step that is a multiple of N, and after the last step (0 = only after "
+                         "the last step)")
     args = ap.parse_args(argv)
+    if args.eval_data and args.model not in ("gpt2", "gpt2-tiny"):
+        ap.error(f"--eval-data evaluates GPT-2 models only, not {args.model}")
+    if args.eval_data and args.gemm != "wgmma":
+        ap.error("--eval-data needs --gemm wgmma: the evaluation loss is computed in the wgmma logits GEMM's epilogue")
+    if args.eval_samples < 0 or args.eval_every < 0:
+        ap.error("--eval-samples and --eval-every cannot be negative")
+    if (args.eval_samples or args.eval_every) and not args.eval_data:
+        ap.error("--eval-samples and --eval-every need --eval-data")
     if args.global_batch < 0 or args.global_batch % args.batch:
         ap.error(f"--global-batch {args.global_batch} is not a multiple of --batch {args.batch}")
     if args.global_batch and os.environ.get("AITJ_ALLREDUCE") == "mc":
