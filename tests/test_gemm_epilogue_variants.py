@@ -15,8 +15,6 @@ import kernel_emulation as ke
 from test_gemm_sass import gemm_sass  # noqa: F401  (module fixture: name -> SASS lines of every GEMM instantiation)
 from trainingjob_operator_b200.ops import functional as F
 
-# gemm_bf16_wgmma_kernel<kBN, kAMN, kBMN, kCM, kEpi>, mangled
-_ARGS = re.compile(r"gemm_bf16_wgmma_kernelILi(\d+)ELb([01])ELb([01])ELi(\d+)ELi(\d+)E")
 # A plain-store or bias epilogue compiles to under 1,100 instructions and the largest variant without GELU (the
 # owner-sharded weight gradient, which looks up the owner of every element) to about 4,700; GELU and dGELU add one
 # MUFU.TANH per output element, and the dGELU + column-sum variant is about 5,900.  The budgets leave room for compiler
@@ -36,11 +34,16 @@ def variants(gemm_sass):  # noqa: F811
     """(block_n, a_mn, b_mn, cluster size, epilogue bits) -> opcodes of that instantiation."""
     out = {}
     for name, lines in gemm_sass.items():
-        m = _ARGS.search(name)
-        assert m, f"{name}: the GEMM kernel has no epilogue template parameter"
-        bn, amn, bmn, cm, epi = (int(g) for g in m.groups())
-        out[(bn, bool(amn), bool(bmn), cm, epi)] = [_opcode(s) for s in lines]
+        keys = ke.gemm_kernel_keys([name])
+        assert keys, f"{name}: the GEMM kernel has no epilogue template parameter"
+        out[keys.pop()] = [_opcode(s) for s in lines]
     return out
+
+
+def test_the_emulated_kernel_table_is_the_compiled_one(variants):
+    """The GEMM stand-in refuses (-7) what the built library has no kernel for; it reads the instantiations from the
+    library's registered kernel names, which must be the ones compiled here."""
+    assert ke.compiled_gemm_kernels() == set(variants)
 
 
 def _gelu(epi):

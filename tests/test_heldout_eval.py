@@ -1,8 +1,8 @@
 """Held-out evaluation of GPT-2 workers (``--eval-data``): the cross-entropy epilogue of the logits GEMM (``EPI_XENT``,
 ``gemm_xent`` + ``xent_finish``), ``GPT2Engine.eval_forward``, the worker's sample assignment, schedule and reports.
 
-CPU tests run the engine with the kernel entry points emulated (``tests/kernel_emulation.py``, plus the two entry points
-of this feature below, which keep the kernels' partial layout) and gloo between processes; the GPU tests run the
+CPU tests run the engine with the kernel entry points emulated (``tests/kernel_emulation.py``, whose ``gemm_xent`` /
+``xent_finish`` keep the kernels' partial layout) and gloo between processes; the GPU tests run the
 hand-written kernels on an H100."""
 import io
 import json
@@ -29,41 +29,12 @@ TESTS = os.path.dirname(os.path.abspath(__file__))
 
 
 # ------------------------------------------------------------------------------------ emulated entry points
-XENT_CALLS = []
-
-
-def gemm_xent(x, w, target, vocab, part, tgt_logit, block_n=0):
-    """What the EPI_XENT kernel stores: per (row, 128-column block) (max, sum of exp(z - max)) over the columns below
-    ``vocab``, and the target's logit, for the rows with a target; the other rows are left as they were."""
-    XENT_CALLS.append(block_n)
-    assert x.dtype == torch.bfloat16 and w.dtype == torch.bfloat16 and block_n in (0, 128, 256, 512, 1024)
-    z = x.float() @ w.float().t()
-    M, N = z.shape
-    nb = F.xent_blocks(N)
-    assert tuple(part.shape) == (M, nb, 2) and 0 < vocab <= N
-    zp = torch.full((M, nb * 128), float("-inf"))
-    zp[:, :vocab] = z[:, :vocab]
-    zb = zp.view(M, nb, 128)
-    mx = zb.max(2).values
-    s = torch.exp(zb - torch.where(torch.isinf(mx), torch.zeros_like(mx), mx)[..., None]).sum(2)
-    live = target >= 0
-    part[live] = torch.stack([mx, s], 2)[live]
-    tgt_logit[live] = z[live].gather(1, target[live][:, None])[:, 0]
-
-
-def xent_finish(part, tgt_logit, target, loss, acc):
-    m, s = part[..., 0], part[..., 1]
-    live = target >= 0
-    mm = torch.where(s > 0, m, torch.full_like(m, float("-inf"))).max(1).values
-    mm = torch.where(live, mm, torch.zeros_like(mm))
-    tot = torch.where(s > 0, s * torch.exp(m - mm[:, None]), torch.zeros_like(s)).sum(1)
-    nll = torch.where(live, mm + torch.log(tot) - tgt_logit, torch.zeros_like(mm))
-    loss.copy_(nll)
-    acc[0] += nll.double().sum()
-    acc[1] += float(live.sum())
+XENT_CALLS = ke.XENT_CALLS
+gemm_xent, xent_finish = ke.gemm_xent, ke.xent_finish
 
 
 def install_xent(monkeypatch=None):
+    """The cross-entropy entry points alone (``kernel_emulation.install`` includes them)."""
     for name, fn in (("gemm_xent", gemm_xent), ("xent_finish", xent_finish)):
         if monkeypatch is not None:
             monkeypatch.setattr(F, name, fn)

@@ -261,52 +261,9 @@ def test_a_checkpoint_round_trip_restores_the_data_position(tmp_path):
 
 
 # ------------------------------------------------------------------------------------ engine in emulation
-def _doc_allowed(doc_start, B, T, dev):
-    ds = doc_start.view(B, 1, T, 1).long()
-    k = torch.arange(T, device=dev).view(1, 1, 1, T)
-    q = torch.arange(T, device=dev).view(1, 1, T, 1)
-    return (k >= ds) & (k <= q)
-
-
-def _attention_fwd_docs(qkv, out, lse, B, T, H, causal=True, scale=0.0, doc_start=None):
-    if doc_start is None:
-        return ke.attention_fwd(qkv, out, lse, B, T, H, causal=causal, scale=scale)
-    ke.CALLS["n"] += 1
-    assert causal and doc_start.dtype == torch.int32 and doc_start.numel() == B * T
-    q, k, v = ke._qkv_heads(qkv, B, T, H)
-    s = ((q @ k.transpose(-1, -2)) * (scale or 0.125)).masked_fill(~_doc_allowed(doc_start, B, T, qkv.device),
-                                                                   float("-inf"))
-    lse.view(B, H, T).copy_(torch.logsumexp(s, -1))
-    out.view(B, T, H, 64).copy_((torch.softmax(s, -1) @ v).transpose(1, 2))
-    return out
-
-
-def _attention_bwd_docs(qkv, out, d_out, lse, delta, dq_acc, d_qkv, B, T, H, causal=True, scale=0.0, doc_start=None):
-    if doc_start is None:
-        return ke.attention_bwd(qkv, out, d_out, lse, delta, dq_acc, d_qkv, B, T, H, causal=causal, scale=scale)
-    ke.CALLS["n"] += 1
-    assert causal and float(dq_acc.abs().max()) == 0.0
-    q, k, v = (t.requires_grad_(True) for t in ke._qkv_heads(qkv, B, T, H))
-    with torch.enable_grad():
-        o = torch.nn.functional.scaled_dot_product_attention(q, k, v, attn_mask=_doc_allowed(doc_start, B, T, qkv.device),
-                                                             scale=(scale or None))
-        grads = torch.autograd.grad(o, (q, k, v), d_out.view(B, T, H, 64).transpose(1, 2).float())
-    dst = d_qkv.view(B, T, 3, H, 64)
-    for i, g in enumerate(grads):
-        dst[:, :, i].copy_(g.transpose(1, 2))
-    return d_qkv
-
-
 def install_doc_attention(monkeypatch=None):
-    """``kernel_emulation.install`` plus attention entry points that also take the document mask."""
-    from trainingjob_operator_b200.ops import functional as F
-
+    """``kernel_emulation.install``: its attention entry points also take the document mask."""
     ke.install(monkeypatch)
-    for name, fn in (("attention_fwd", _attention_fwd_docs), ("attention_bwd", _attention_bwd_docs)):
-        if monkeypatch is not None:
-            monkeypatch.setattr(F, name, fn)
-        else:
-            setattr(F, name, fn)
 
 
 def _doc_batch(B, T, vocab, eot, seed):

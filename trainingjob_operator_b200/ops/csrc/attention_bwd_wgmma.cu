@@ -317,6 +317,8 @@ int aitj_attn_bwd(const void* qkv, const void* out, const void* d_out, const voi
   if (T % 128) return -1;
   if (doc_start && !causal) return -5;
   if (reinterpret_cast<uintptr_t>(doc_start) & 7) return -4;   // read as int2 pairs
+  // qkv and d_out are read by TMA: refused here by name rather than by the tensor-map encoder's error
+  if ((reinterpret_cast<uintptr_t>(qkv) & 15) || (reinterpret_cast<uintptr_t>(d_out) & 15)) return -4;
   const int C = H * AB_D;
   const uint64_t rows = static_cast<uint64_t>(B) * T;
   CUtensorMap tq, tdo;

@@ -867,10 +867,10 @@ int aitj_norm_share(void* parts_mc, const void* mine, int rank, void* stream) {
 int aitj_adamw(void* p, void* g, void* m, void* v, void* p16, const void* wd_mask, const void* sumsq,
                const void* dyn, long long n, float lr, float beta1, float beta2, float eps, float weight_decay, int step, float max_norm,
                float grad_div, int zero_grad, void* stream) {
-  if (n % 256) return -1;
   AdamArgs a;
   a.sumsq_n = g_adam_sumsq_n; a.p16_mc = g_adam_p16_mc;
-  g_adam_sumsq_n = 1; g_adam_p16_mc = 0;
+  g_adam_sumsq_n = 1; g_adam_p16_mc = 0;   // taken before the refusal: a refused sweep does not pass them on
+  if (n % 256) return -1;
   a.lr = lr; a.beta1 = beta1; a.beta2 = beta2; a.eps = eps; a.weight_decay = weight_decay;
   a.bc1 = 1.0f - powf(beta1, static_cast<float>(step));
   a.bc2 = 1.0f - powf(beta2, static_cast<float>(step));

@@ -685,8 +685,11 @@ int aitj_gemm_bf16(const void* A, const void* B, void* out, int M, int N, int K,
                    int a_mn, int b_mn, const void* bias, const void* residual, void* aux, int flags, int split_k,
                    int block_n, int max_ctas, void* stream_ptr) {
   using namespace aitj;
+  // both one-shot buffers are taken before any refusal, so that a refused call cannot hand them to the next GEMM
   const auto xent = g_gemm_xent;
   g_gemm_xent = {nullptr, nullptr, nullptr, 0};
+  float* const colsum = g_gemm_colsum;
+  g_gemm_colsum = nullptr;
   if (flags & EPI_XENT) {
     // the max and the sum of exponentials of a row cannot be formed from the partial products of a K split
     if (flags != EPI_XENT || split_k > 1 || !xent.target || !xent.part || !xent.tgt || xent.vocab < 1 ||
@@ -715,8 +718,7 @@ int aitj_gemm_bf16(const void* A, const void* B, void* out, int M, int N, int K,
   args.bias = reinterpret_cast<const __nv_bfloat16*>(bias);
   args.residual = reinterpret_cast<const __nv_bfloat16*>(residual);
   args.aux = reinterpret_cast<__nv_bfloat16*>(aux);
-  args.colsum = g_gemm_colsum;
-  g_gemm_colsum = nullptr;
+  args.colsum = colsum;
   if (args.colsum && (flags & (EPI_OUT_F32 | EPI_ACCUM | EPI_XENT))) return -6;   // column sums of a bf16 output only
   args.xent_target = xent.target;
   args.xent_part = xent.part;
