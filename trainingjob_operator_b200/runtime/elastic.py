@@ -20,6 +20,8 @@ from typing import Any, Dict, Optional
 import torch
 import torch.distributed as dist
 
+from .rendezvous import guarded
+
 ANN_METRICS = "aitj.b200/metrics"
 ANN_WORKER_TRACE = "aitj.b200/worker-trace"
 ANN_RESCALE = "aitj.b200/rescale-trace"
@@ -145,16 +147,9 @@ class ElasticWatcher:
         newest = mine
         if dist.is_initialized() and dist.get_world_size() > 1:
             t = torch.tensor([mine], dtype=torch.int64, device=device if device.type == "cuda" else "cpu")
-            if guard is not None:
-                guard.in_step = True
-            try:
+            with guarded(guard, "the generation agreement"):
                 dist.all_reduce(t, op=dist.ReduceOp.MAX)
                 newest = int(t[0])
-            finally:
-                if guard is not None:
-                    guard.in_step = False
-            if guard is not None and guard.tripped:
-                raise RuntimeError("the communicator was aborted while the generation agreement was in flight")
         if newest <= self.generation:
             return None
         return self._wait_for(newest)

@@ -8,6 +8,7 @@ The reference has none of this: it starts N containers with a fixed environment 
 """
 from __future__ import annotations
 
+import contextlib
 import gc
 import os
 import threading
@@ -330,3 +331,23 @@ class StallBreaker:
 
     def stop(self) -> None:
         self._stop.set()
+
+
+@contextlib.contextmanager
+def guarded(breaker, what: str, generation: Optional[int] = None):
+    """Run the body as "inside a step" for ``breaker`` (a StallBreaker; None: the body runs as is): a collective in it
+    that hangs behind a dead peer gets the communicator aborted, and the abort surfaces here as a RuntimeError naming
+    ``what``, which the training loop's recovery path handles.  ``generation``: the body starts at a step boundary of it
+    -- only a newer generation (another peer lost meanwhile) makes the breaker abort."""
+    if breaker is None:
+        yield
+        return
+    if generation is not None:
+        breaker.progress(generation)
+    breaker.in_step = True
+    try:
+        yield
+    finally:
+        breaker.in_step = False
+    if breaker.tripped:
+        raise RuntimeError(f"the communicator was aborted while {what} was in flight")

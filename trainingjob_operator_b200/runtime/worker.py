@@ -32,9 +32,10 @@ from typing import Any, Dict, List, Optional
 import torch
 import torch.distributed as dist
 
+from ..ops import lib as oplib
 from .elastic import ElasticWatcher, env_int, rendezvous_from_env
-from .rendezvous import (StaleGeneration, StallBreaker, heartbeat, init_process_group, max_over_ranks,  # noqa: F401
-                         rendezvous, sync_state, teardown_group, wait_for_newer_generation)
+from .rendezvous import (StaleGeneration, StallBreaker, guarded, heartbeat, init_process_group,  # noqa: F401
+                         max_over_ranks, rendezvous, sync_state, teardown_group, wait_for_newer_generation)
 from .trainer import EngineTrainer, SyntheticTokens
 
 
@@ -210,10 +211,17 @@ class EngineAdapter:
             self.trainer.step_count = v
 
     def launches_per_step(self) -> int:
+        return self.trainer.launches_per_step or 0
+
+    @property
+    def gradient_sync(self) -> str:
+        return self.trainer.allreduce_backend
+
+    def graph_report(self, world: int) -> Dict[str, Any]:
+        """The result's CUDA-graph and all-reduce fields."""
         t = self.trainer
-        if t.launches_per_step:
-            return t.launches_per_step
-        return 0
+        return {"cuda_graph": bool(t.graph or t.seg_graphs), "graph_segments": len(t.seg_graphs or []) or None,
+                "graph_error": t.graph_error, "allreduce": t.allreduce_backend}
 
 
 class TorchAdapter:
@@ -393,6 +401,13 @@ class TorchAdapter:
     def launches_per_step(self) -> int:
         return 1 if self.dev.type == "cuda" else 0
 
+    gradient_sync = "flat buffer all-reduce (nccl / gloo)"
+
+    def graph_report(self, world: int) -> Dict[str, Any]:
+        """The result's CUDA-graph and all-reduce fields."""
+        return {"cuda_graph": bool(self.graph), "graph_segments": None, "graph_error": self.graph_error,
+                "allreduce": "nccl" if world > 1 else "none"}
+
 
 def build_adapter(args, device: torch.device):
     if args.model in ("gpt2", "gpt2-tiny", "bert", "bert-tiny"):
@@ -449,23 +464,6 @@ def load_checkpoint(args, adapter) -> int:
     return int(meta["step"])
 
 
-def guarded(breaker, generation: int, fn):
-    """Run a collective-bearing ``fn`` as "inside a step" for the stall breaker: only a generation newer than
-    ``generation`` (= another peer was lost meanwhile) makes it abort the communicator; the abort surfaces as a
-    RuntimeError, which the training loop's recovery path handles."""
-    if breaker is None:
-        return fn()
-    breaker.progress(generation)
-    breaker.in_step = True
-    try:
-        out = fn()
-    finally:
-        breaker.in_step = False
-    if breaker.tripped:
-        raise RuntimeError("the communicator was aborted while the state hand-off was in flight")
-    return out
-
-
 # ------------------------------------------------------------------------------------ main loop
 def dump_outputs(out_dir: str, adapter, losses) -> None:
     """What the timed steps computed, so that two builds can be compared output for output on the same seeded inputs:
@@ -485,414 +483,431 @@ def dump_outputs(out_dir: str, adapter, losses) -> None:
     np.save(os.path.join(out_dir, "weights_sample.npy"), w.float().cpu().numpy())
 
 
-def run(args) -> Dict[str, Any]:
-    t_proc = time.time()
-    rank = env_int("RANK", env_int("TRAININGJOB_REPLICA_INDEX", 0))
-    rdv = rendezvous_from_env()
-    world, port, generation = rdv["world"], rdv["port"], rdv["generation"]
-    use_cuda = torch.cuda.is_available() and not args.cpu
-    device = torch.device("cuda", env_int("LOCAL_RANK", 0) if torch.cuda.device_count() > 1 else 0) \
-        if use_cuda else torch.device("cpu")
-    if use_cuda:
-        torch.cuda.set_device(device)
-    if args.elastic and os.environ.get("AITJ_FAULT_TOLERANT") == "1":
-        # NCCL's watchdog would take the process down on an asynchronous communicator error or a collective timeout
-        # (TearDown / SkipCleanUp); a faultTolerant job handles the loss of a peer itself (StallBreaker + recovery below)
-        os.environ.setdefault("TORCH_NCCL_ASYNC_ERROR_HANDLING", "0")
-        # A communicator that must be abortable with a peer already dead should not hold NVSwitch multicast (NVLS)
-        # objects: their teardown involves every member.  Precaution, not a measured fix.  Costs the faultTolerant job's
-        # all-reduce the in-switch reduction.
-        os.environ.setdefault("NCCL_NVLS_ENABLE", "0")
-    trace = {"process_start": t_proc, "torch_imported": time.time()}
-    heartbeat(force=True)
-    watcher = ElasticWatcher.from_env(generation)
-    if watcher is not None and not args.elastic:
-        watcher.poll = 5.0  # reporting only
-    adapter = build_adapter(args, device)
-    trace["model_built"] = time.time()
-    heartbeat(force=True)
-    joiner = bool(args.elastic and watcher is not None and generation > 1 and world > 1)
-    if joiner:
-        # Joining a running job: do everything that needs no peer first -- CUDA context, model build, two throw-away
-        # steps (kernel loading, cuDNN plans, allocator growth; the state is overwritten by rank 0's broadcast
-        # anyway) -- and only then tell the survivors, who keep training until this rank is ready to rendezvous.
-        adapter.bind(None, warm_up=True)     # single-micro-batch steps: not 2k micro-batches of throw-away work
-        for _ in range(2):
-            adapter.train_step()
-        if use_cuda:
+class _Left(Exception):
+    """This rank is not part of the job's new world: ``run`` returns the record it carries."""
+
+
+class _TimedRegion:
+    """The measured steps, bracketed by barrier + synchronize and CUDA events, with the evaluations that ran inside it
+    (device ms, wall ms, kernel launches) taken out of the step figures."""
+
+    def __init__(self, use_cuda: bool):
+        self.use_cuda = use_cuda
+        self.from_step = -1          # first step inside the region (-1: not armed yet)
+        self.eval_ms = self.eval_wall_ms = 0.0
+        self.eval_launches = 0
+
+    def arm(self, step: int, world: int) -> None:
+        if world > 1:
+            dist.barrier()
+        if self.use_cuda:
             torch.cuda.synchronize()
-        trace["prewarmed"] = time.time()
-        watcher.announce_ready(rank, generation)
-        print(f"[worker {rank}] joiner ready for generation {generation} after "
-              f"{trace['prewarmed'] - t_proc:.2f}s of local set-up (model build "
-              f"{trace['model_built'] - t_proc:.2f}s, warm-up steps {trace['prewarmed'] - trace['model_built']:.2f}s)",
-              flush=True)
-    if world > 1:
-        got = rendezvous(rank, {"generation": generation, "world": world, "port": port}, device, watcher)
-        if got is None:
-            print(f"[worker {rank}] not part of the current world any more, leaving", flush=True)
-            return {"left": True, "generation": generation, "step": 0}
-        generation, world, port = got["generation"], got["world"], got["port"]
-        if watcher is not None:
-            watcher.adopted(generation, world)
-    trace["rendezvous_done"] = time.time()
-    heartbeat(force=True)
-    adapter.bind(None)
-    print(f"[worker {rank}] world {world}: gradient sync = "
-          f"{getattr(getattr(adapter, 'trainer', None), 'allreduce_backend', 'flat buffer all-reduce (nccl / gloo)')}",
-          flush=True)
+            self.ev0, self.ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            self.ev0.record()
+        self.t_wall0, self.t_epoch0 = time.perf_counter(), time.time()
+        self.from_step = step
+        self.launches0 = oplib.LAUNCHES
 
-    restart_count = env_int("TRAININGJOB_REPLICA_RESTARTCOUNT", 0)
-    start_step = 0
-    if restart_count > 0 and args.ckpt_every > 0:
-        start_step = load_checkpoint(args, adapter)
-        adapter.step_count = start_step
-        print(f"[worker {rank}] restart #{restart_count}: resumed from checkpoint at step {start_step}"
-              + (f", data position {adapter.data_position}" if hasattr(adapter, "data_position") else ""), flush=True)
-    # a joiner without a checkpoint only has its throw-away warm-up state: it must never be elected as the source
-    joined_step = sync_state(adapter, start_step, device, have_state=not joiner or start_step > 0)
-    if joiner:
-        print(f"[worker {rank}] joined generation {generation} (world {world}) at step {joined_step}", flush=True)
-    # faultTolerant (types.go:47, never read by the reference): the loss of a peer is survived in place -- see the
-    # except branch of the training loop
-    fault_tolerant = bool(args.elastic and watcher is not None and os.environ.get("AITJ_FAULT_TOLERANT") == "1")
-    breaker = None
-    # (armed on CUDA, where a collective with a dead peer hangs instead of raising; AITJ_STALL_BREAKER=force arms it for
-    #  any backend -- the CPU tests use it with collectives that are made to hang the way NCCL's do)
-    hangs = use_cuda or os.environ.get("AITJ_STALL_BREAKER") == "force"
-    if fault_tolerant and hangs and float(os.environ.get("AITJ_FT_ABORT_AFTER", "3")) > 0:
-        breaker = StallBreaker(watcher, float(os.environ.get("AITJ_FT_ABORT_AFTER", "3")))
-    elif watcher is not None and hangs and world > 1 and float(os.environ.get("AITJ_STALL_EXIT_AFTER", "3")) > 0:
-        # not faultTolerant: a rank stuck behind a dead peer cannot be repaired in place; once the controller has started
-        # to repair the job (newer generation) it leaves at once instead of waiting for the heartbeat time-out
-        breaker = StallBreaker(watcher, float(os.environ.get("AITJ_STALL_EXIT_AFTER", "3")), action="exit")
-    recoveries: List[Dict[str, Any]] = []
+    def exclude(self, ms: float, wall_ms: float, launches: int) -> None:
+        """An evaluation ran: out of the step figures if it was inside the region."""
+        if self.from_step >= 0:
+            self.eval_ms += ms
+            self.eval_wall_ms += wall_ms
+            self.eval_launches += launches
 
-    stop = {"flag": False}
-    signal.signal(signal.SIGTERM, lambda *_: stop.__setitem__("flag", True))
-
-    total = args.warmup + args.steps if args.steps > 0 else 1 << 60
-    losses: List[float] = []
-    rescales: List[Dict[str, Any]] = []
-    timing: Dict[str, Any] = {}
-    ev0 = ev1 = None
-    t_wall0 = 0.0
-    t_epoch0 = 0.0
-    timed_from = -1          # first step inside the timed region (-1: not armed yet)
-    step = joined_step
-    first_step_done = False
-    pending_rescale = None
-    from ..ops import lib as oplib
-
-    launches0 = 0
-    # rank 0 publishes its wall-clock throughput every AITJ_REPORT_EVERY seconds (0 = only the final, device-timed result)
-    report_every = float(os.environ.get("AITJ_REPORT_EVERY", "10"))
-    live_t0, live_step0 = time.time(), step
-    # held-out evaluation (--eval-data): at the boundary before every step that is a multiple of --eval-every, and once
-    # after the last step.  A boundary's evaluation is done once it has completed.  Every (re-)bind to a new generation
-    # forgets that (last_eval_step = -1): a joiner knows nothing of it, so after a rescale or a recovery at a boundary
-    # that was already evaluated -- a peer lost in the step right after an evaluation -- every rank of the new generation
-    # evaluates it again, and all of them issue the same collectives.
-    evals: List[Dict[str, Any]] = []
-    last_eval_step = -1
-    # evaluation inside the timed region (device ms, wall ms, kernel launches), taken out of the step figures; and the
-    # evaluation wall time since the last interim report, taken out of its throughput
-    eval_ms_timed = eval_wall_timed = 0.0
-    eval_launches_timed = 0
-    live_eval_s = 0.0
-
-    def eval_due(s: int) -> bool:
-        if not hasattr(adapter, "eval_data") or s == last_eval_step:
-            return False
-        return (s > 0 and args.eval_every > 0 and s % args.eval_every == 0) or (args.steps > 0 and s >= total)
-
-    while (step < total or eval_due(step)) and not stop["flag"]:
-        if breaker is not None:
-            breaker.progress(generation)
-            # patience from this generation's completed steps: the first step on a freshly bound trainer captures CUDA
-            # graphs / loads kernels, and an accumulated step can take seconds -- neither is a stall
-            breaker.begin_step(generation)
-        failure = None
-        try:
-            # ---- elastic: agree on the newest rendezvous generation at the step boundary ------------
-            if watcher is not None and args.elastic:
-                target = watcher.agree(device, guard=breaker)
-                if target is not None and target["generation"] != generation:
-                    t0 = time.time()
-                    new_world = target["world"]
-                    print(f"[worker {rank}] rendezvous generation {generation} -> {target['generation']} "
-                          f"(world {world} -> {new_world}) at step {step}", flush=True)
-                    if dist.is_initialized():
-                        adapter.prepare_state()       # sharded optimizer state -> whole state on every survivor
-                        if use_cuda:
-                            torch.cuda.synchronize()
-                        dist.destroy_process_group()
-                    if rank >= new_world:
-                        print(f"[worker {rank}] leaving: world shrinks to {new_world} (generation {target['generation']})",
-                              flush=True)
-                        return {"left": True, "generation": target["generation"], "step": step}
-                    generation, world, port = target["generation"], new_world, target["port"]
-                    t1 = time.time()
-                    if world > 1:
-                        got = rendezvous(rank, {"generation": generation, "world": world, "port": port}, device, watcher)
-                        if got is None:
-                            return {"left": True, "generation": generation, "step": step}
-                        generation, world, port = got["generation"], got["world"], got["port"]
-                    t2 = time.time()
-                    adapter.bind(None)
-                    last_eval_step = -1
-                    step = guarded(breaker, generation, lambda: sync_state(adapter, step, device))
-                    heartbeat(force=True)
-                    watcher.adopted(generation, world)
-                    pending_rescale = {"generation": generation, "world": world, "t0": t0,
-                                       "observed_at": target.get("observed_at", t0),
-                                       "teardown_s": t1 - t0, "init_pg_s": t2 - t1, "sync_state_s": time.time() - t2}
-                    continue    # back to the step boundary: every rank (joiners included) runs the same sequence
-            # ---- timed region bookkeeping ----------------------------------------------------------------
-            # armed at the first step boundary at or past the warm-up: a replica resumed from a checkpoint (or an
-            # elastic joiner) starts past `--warmup` and still gets a timed region (and counts the steps it timed)
-            if timed_from < 0 and step >= args.warmup and args.steps > 0:
-                if world > 1:
-                    dist.barrier()
-                if use_cuda:
-                    torch.cuda.synchronize()
-                    ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                    ev0.record()
-                t_wall0 = time.perf_counter()
-                t_epoch0 = time.time()
-                timed_from = step
-                launches0 = oplib.LAUNCHES
-            if eval_due(step):
-                if breaker is not None:
-                    breaker.progress(generation)
-                    breaker.in_step = True
-                t_eval = time.perf_counter()
-                launches_before = oplib.LAUNCHES
-                e0 = e1 = None
-                if use_cuda:
-                    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                    e0.record()
-                try:
-                    # an evaluation is as long as its micro-batches make it: the stall breaker sees progress after each
-                    # one, not the patience of a single training step for the whole of it
-                    rec = adapter.evaluate(progress=None if breaker is None else lambda: breaker.progress(generation))
-                finally:
-                    if breaker is not None:
-                        breaker.in_step = False
-                if breaker is not None and breaker.tripped:
-                    raise RuntimeError("the communicator was aborted while an evaluation was in flight")
-                wall_ms = (time.perf_counter() - t_eval) * 1e3
-                if use_cuda:
-                    e1.record()
-                    e1.synchronize()
-                ms = e0.elapsed_time(e1) if use_cuda else wall_ms
-                if timed_from >= 0:
-                    eval_ms_timed += ms
-                    eval_wall_timed += wall_ms
-                    eval_launches_timed += oplib.LAUNCHES - launches_before
-                live_eval_s += wall_ms / 1e3
-                rec = {"step": step, "loss": rec["loss"], "tokens": rec["tokens"], "samples": rec["samples"],
-                       "ms": round(ms, 3)}
-                evals.append(rec)
-                last_eval_step = step
-                if rank == 0:
-                    print(f"[worker {rank}] step {step}: eval loss {rec['loss']:.6f} over {rec['samples']} held-out "
-                          f"windows ({rec['tokens']} tokens) in {ms:.1f} ms", flush=True)
-                if step >= total:
-                    continue          # the evaluation after the last step: the loop ends here
-            if breaker is not None:
-                breaker.progress(generation)
-                breaker.in_step = True
-            t_step = time.perf_counter()
-            try:
-                loss = adapter.train_step()
-            finally:
-                if breaker is not None:
-                    breaker.in_step = False
-            if breaker is not None:
-                breaker.step_done(generation, time.perf_counter() - t_step)
-            if breaker is not None and breaker.tripped:
-                raise RuntimeError("the communicator was aborted while this step was in flight")
-        except RuntimeError as e:
-            # ---- faultTolerant: a peer died under a collective -----------------------------------------------------
-            # (gloo raises in the survivors; for NCCL the StallBreaker aborts the communicator.)  The survivors keep
-            # their process, device state and -- on GPUs -- CUDA context: drop the broken group, wait for the
-            # controller to replace the lost replica (restart scope Pod, new rendezvous generation), re-rendezvous and
-            # continue from the survivors' state.  Without faultTolerant the error ends this replica and the job's
-            # restartPolicy / restartScope take over, as in the reference (pod.go:208-250).
-            if not fault_tolerant or world <= 1:
-                raise
-            failure = (type(e).__name__, (str(e).splitlines() or [""])[0][:160])
-        if failure is not None:
-            # (outside the except block: the traceback of the failed step references the work handles of the broken
-            # group, and with them its sockets)
-            t0 = time.time()
-            aborted = breaker is not None and breaker.tripped
-            print(f"[worker {rank}] step {step}: lost a peer ({failure[0]}: {failure[1]}); "
-                  f"keeping state, waiting for the next rendezvous generation", flush=True)
-            # pending work handles keep the group's sockets open; a peer that is blocked on *us* (gloo does not
-            # propagate a failure beyond the dead rank's direct neighbours) only errors out once they really close
-            adapter.discard_step()
-            teardown_group(broken=True)
-            gc.collect()
-            target = wait_for_newer_generation(watcher, generation, float(os.environ.get("AITJ_FT_WAIT", "120")),
-                                               should_stop=lambda: stop["flag"])
-            if target is None and stop["flag"]:
-                print(f"[worker {rank}] terminated while waiting for the job to be repaired", flush=True)
-                break
-            if target is None:
-                print(f"[worker {rank}] no new rendezvous generation was published: giving up", flush=True)
-                raise RuntimeError(f"collective failed and the job was not repaired: {failure[0]}: {failure[1]}")
-            if rank >= target["world"]:
-                print(f"[worker {rank}] leaving: world shrinks to {target['world']} (generation {target['generation']})",
-                      flush=True)
-                return {"left": True, "generation": target["generation"], "step": step}
-            t1 = time.time()
-            got = rendezvous(rank, {"generation": target["generation"], "world": target["world"],
-                                    "port": target["port"]}, device, watcher)
-            if got is None:
-                return {"left": True, "generation": target["generation"], "step": step}
-            generation, world, port = got["generation"], got["world"], got["port"]
-            t2 = time.time()
-            if aborted and args.ckpt_every > 0 and os.path.exists(ckpt_path(args)):
-                # kernels released by an abort ran on with whatever the dead peer left in the buffers: do not trust
-                # this rank's copy when there is a checkpoint to fall back to
-                step = load_checkpoint(args, adapter)
-                adapter.step_count = step
-            if breaker is not None:
-                breaker.tripped = False
-                breaker.progress(generation)
-            adapter.bind(None)
-            last_eval_step = -1
-            # the hand-off is a chain of collectives on the new group: if ANOTHER peer dies under it, a still newer
-            # generation is published and the breaker must be able to get this rank out of it
-            try:
-                step = guarded(breaker, generation, lambda: sync_state(adapter, step, device))
-            except RuntimeError as e:
-                # (this block is outside the loop's try: handled here.)  The group is gone again; the step boundary's
-                # generation agreement finds the newest record and joins it through the ordinary rescale path.
-                print(f"[worker {rank}] another peer was lost during the state hand-off of generation {generation} "
-                      f"({type(e).__name__}); joining the next generation", flush=True)
-                teardown_group(broken=True)
-                if breaker is not None:
-                    breaker.tripped = False
-                continue
-            heartbeat(force=True)
-            watcher.adopted(generation, world)
-            pending_rescale = {"generation": generation, "world": world, "t0": t0, "observed_at": t0,
-                               "teardown_s": t1 - t0, "init_pg_s": t2 - t1, "sync_state_s": time.time() - t2,
-                               "recovered_from": failure[0]}
-            continue
-        losses.append(loss)
-        step += 1
-        heartbeat()
-        if pending_rescale is not None:
-            # the first completed step at the new world size ends the rescale
-            now = time.time()
-            rec = {"generation": pending_rescale["generation"], "world": pending_rescale["world"],
-                   "seconds": now - pending_rescale["t0"], "since_change": now - pending_rescale["observed_at"],
-                   "teardown_s": round(pending_rescale["teardown_s"], 4),
-                   "init_pg_s": round(pending_rescale["init_pg_s"], 4),
-                   "sync_state_s": round(pending_rescale["sync_state_s"], 4)}
-            rec["first_step_s"] = round(rec["seconds"] - rec["teardown_s"] - rec["init_pg_s"] - rec["sync_state_s"], 4)
-            if "recovered_from" in pending_rescale:
-                rec["recovered_from"] = pending_rescale["recovered_from"]
-                recoveries.append(rec)
-            rescales.append(rec)
-            print(f"[worker {rank}] step {step}: rescaled to world={rec['world']} gen={rec['generation']} in "
-                  f"{rec['seconds']:.3f}s", flush=True)
-            if watcher is not None:
-                watcher.report_rescale(rank, rec, force="recovered_from" in rec)   # rank 0 may be the replaced one
-            pending_rescale = None
-        if not first_step_done:
-            first_step_done = True
-            trace["first_step_done"] = time.time()
-            if watcher is not None:
-                watcher.report_trace(rank, trace)
-        if rank == 0 and watcher is not None and report_every > 0 and time.time() - live_t0 >= report_every:
-            dt, n = time.time() - live_t0 - live_eval_s, step - live_step0
-            if n > 0 and dt > 0:
-                G = adapter.plan.global_batch
-                live = {"samples_per_sec": round(G * n / dt, 2), "ms_per_step": round(dt * 1e3 / n, 3), "world": world,
-                        "steps_done": step, "global_batch": G, "recoveries": len(recoveries)}
-                if evals:
-                    live.update(eval_loss=evals[-1]["loss"], eval_step=evals[-1]["step"])
-                watcher.report_live(rank, live)
-            live_t0, live_step0, live_eval_s = time.time(), step, 0.0
-        if args.ckpt_every > 0 and step % args.ckpt_every == 0:
-            adapter.prepare_state()
-            if rank == 0:
-                save_checkpoint(args, adapter, adapter.step_count)
-        if args.step_sleep > 0:
-            time.sleep(args.step_sleep)
-
-    result: Dict[str, Any] = {"rank": rank, "world": world, "steps_done": step, "generation": generation,
-                              "final_loss": losses[-1] if losses else None, "rescales": rescales,
-                              "recoveries": recoveries, "trace": trace}
-    if hasattr(adapter, "data_position"):
-        result["data_position"] = adapter.data_position
-    if hasattr(adapter, "eval_data"):
-        result.update(evals=evals, eval_loss_last=evals[-1]["loss"] if evals else None)
-    if breaker is not None:
-        breaker.stop()
-    if _CKPT.get("writer") is not None:
-        _CKPT["writer"].wait(60.0)
-    n_timed = step - timed_from if timed_from >= 0 else 0
-    if args.steps > 0 and step >= total and n_timed > 0:
-        if use_cuda:
-            ev1.record()
+    def close(self, step: int, world: int, device, global_batch: int, graph_launches: int) -> Dict[str, Any]:
+        """Collective, after the last step of an armed region: the timing fields of the result, the device time being
+        the slowest rank's."""
+        n = step - self.from_step
+        if self.use_cuda:
+            self.ev1.record()
             torch.cuda.synchronize()
         t_epoch1 = time.time()
         if world > 1:
             dist.barrier()
-        wall_total = time.perf_counter() - t_wall0
-        dev_ms = (ev0.elapsed_time(ev1) if use_cuda else wall_total * 1e3) - eval_ms_timed
-        wall = wall_total - eval_wall_timed / 1e3
+        wall_total = time.perf_counter() - self.t_wall0
+        dev_ms = (self.ev0.elapsed_time(self.ev1) if self.use_cuda else wall_total * 1e3) - self.eval_ms
+        wall = wall_total - self.eval_wall_ms / 1e3
         dev_ms = max_over_ranks(dev_ms, device)
-        plan = adapter.plan
-        global_batch = plan.global_batch
-        result.update({"timed_steps": n_timed, "timed_from_step": timed_from,
-                       "timed_region_epoch": [t_epoch0, t_epoch1]})
-        graph_launches = adapter.launches_per_step()
-        eager_launches = oplib.LAUNCHES - launches0 - eval_launches_timed
-        result.update({
-            "ms_per_step": dev_ms / n_timed,
-            "samples_per_sec": global_batch * n_timed / (dev_ms / 1e3),
-            "wall_ms_per_step": wall * 1e3 / n_timed,
-            "global_batch": global_batch, "batch_per_gpu": args.batch,
-            "micro_batches": plan.k, "micro_batches_this_rank": plan.n,
-            "h2d_bytes_per_step": adapter.h2d_bytes, "d2h_bytes_per_step": adapter.d2h_bytes,
-            "gpu_launches": graph_launches * n_timed if graph_launches else eager_launches,
-            "launches_per_step": graph_launches or (eager_launches // max(1, n_timed)),
-            "loss_first": losses[0] if losses else None, "loss_last": losses[-1] if losses else None,
-            "flops_per_step": getattr(adapter, "flops_per_step", 0.0) * plan.n,     # this rank's work
-            "describe": adapter.describe,
-            "cuda_graph": bool(getattr(getattr(adapter, "trainer", None), "graph", None)
-                               or getattr(getattr(adapter, "trainer", None), "seg_graphs", None)
-                               or getattr(adapter, "graph", None)),
-            "graph_segments": len(getattr(getattr(adapter, "trainer", None), "seg_graphs", None) or []) or None,
-            "graph_error": getattr(getattr(adapter, "trainer", None), "graph_error", None)
-            or getattr(adapter, "graph_error", None),
-            "allreduce": getattr(getattr(adapter, "trainer", None), "allreduce_backend", "nccl" if world > 1 else "none"),
-        })
-    if args.dump_outputs and n_timed > 0:
-        # collective: with the owner-sharded optimizer each rank keeps only its own range of the master weights current
-        adapter.prepare_state()
-        if rank == 0:
-            dump_outputs(args.dump_outputs, adapter, losses[-n_timed:])
-    if rank == 0 and args.result:
-        os.makedirs(os.path.dirname(os.path.abspath(args.result)), exist_ok=True)
-        with open(args.result + ".tmp", "w") as f:
-            json.dump(result, f)
-        os.replace(args.result + ".tmp", args.result)
-    if rank == 0 and watcher is not None:
-        watcher.report_result(result)
-    if dist.is_initialized():
+        eager_launches = oplib.LAUNCHES - self.launches0 - self.eval_launches
+        return {"timed_steps": n, "timed_from_step": self.from_step, "timed_region_epoch": [self.t_epoch0, t_epoch1],
+                "ms_per_step": dev_ms / n, "samples_per_sec": global_batch * n / (dev_ms / 1e3),
+                "wall_ms_per_step": wall * 1e3 / n,
+                "gpu_launches": graph_launches * n if graph_launches else eager_launches,
+                "launches_per_step": graph_launches or (eager_launches // max(1, n))}
+
+
+class _Loop:
+    """The training loop of one replica and the state it keeps from step to step (``run``)."""
+
+    def __init__(self, args):
+        t_proc = time.time()
+        self.args = args
+        self.rank = env_int("RANK", env_int("TRAININGJOB_REPLICA_INDEX", 0))
+        rdv = rendezvous_from_env()
+        self.world, self.port, self.generation = rdv["world"], rdv["port"], rdv["generation"]
+        self.use_cuda = torch.cuda.is_available() and not args.cpu
+        self.device = torch.device("cuda", env_int("LOCAL_RANK", 0) if torch.cuda.device_count() > 1 else 0) \
+            if self.use_cuda else torch.device("cpu")
+        if self.use_cuda:
+            torch.cuda.set_device(self.device)
+        if args.elastic and os.environ.get("AITJ_FAULT_TOLERANT") == "1":
+            # NCCL's watchdog would take the process down on an asynchronous communicator error or a collective timeout
+            # (TearDown / SkipCleanUp); a faultTolerant job handles the loss of a peer itself (StallBreaker + _recover)
+            os.environ.setdefault("TORCH_NCCL_ASYNC_ERROR_HANDLING", "0")
+            # A communicator that must be abortable with a peer already dead should not hold NVSwitch multicast (NVLS)
+            # objects: their teardown involves every member.  Precaution, not a measured fix.  Costs the faultTolerant
+            # job's all-reduce the in-switch reduction.
+            os.environ.setdefault("NCCL_NVLS_ENABLE", "0")
+        self.trace = {"process_start": t_proc, "torch_imported": time.time()}
+        heartbeat(force=True)
+        self.watcher = watcher = ElasticWatcher.from_env(self.generation)
+        if watcher is not None and not args.elastic:
+            watcher.poll = 5.0  # reporting only
+        self.adapter = build_adapter(args, self.device)
+        self.trace["model_built"] = time.time()
+        heartbeat(force=True)
+        self.step = 0
+        self._join_job()
+        # faultTolerant (types.go:47, never read by the reference): the loss of a peer is survived in place (_recover)
+        self.fault_tolerant = bool(args.elastic and watcher is not None and os.environ.get("AITJ_FAULT_TOLERANT") == "1")
+        self.breaker = None
+        # (armed on CUDA, where a collective with a dead peer hangs instead of raising; AITJ_STALL_BREAKER=force arms it
+        #  for any backend -- the CPU tests use it with collectives that are made to hang the way NCCL's do)
+        hangs = self.use_cuda or os.environ.get("AITJ_STALL_BREAKER") == "force"
+        if self.fault_tolerant and hangs and float(os.environ.get("AITJ_FT_ABORT_AFTER", "3")) > 0:
+            self.breaker = StallBreaker(watcher, float(os.environ.get("AITJ_FT_ABORT_AFTER", "3")))
+        elif watcher is not None and hangs and self.world > 1 and float(os.environ.get("AITJ_STALL_EXIT_AFTER", "3")) > 0:
+            # not faultTolerant: a rank stuck behind a dead peer cannot be repaired in place; once the controller has
+            # started to repair the job (newer generation) it leaves at once instead of waiting for the heartbeat time-out
+            self.breaker = StallBreaker(watcher, float(os.environ.get("AITJ_STALL_EXIT_AFTER", "3")), action="exit")
+        self.stopping = False
+        signal.signal(signal.SIGTERM, lambda *_: setattr(self, "stopping", True))
+        self.total = args.warmup + args.steps if args.steps > 0 else 1 << 60
+        self.losses, self.rescales, self.recoveries = [], [], []
+        # armed at the first step boundary at or past the warm-up: a replica resumed from a checkpoint (or an elastic
+        # joiner) starts past `--warmup` and still gets a timed region (and counts the steps it timed)
+        self.region = _TimedRegion(self.use_cuda)
+        self.pending_rescale: Optional[Dict[str, Any]] = None
+        # rank 0 publishes its wall-clock throughput every AITJ_REPORT_EVERY seconds (0 = only the final, device-timed
+        # result), without the evaluation wall time since the last report
+        self.report_every = float(os.environ.get("AITJ_REPORT_EVERY", "10"))
+        self.live_t0, self.live_step0, self.live_eval_s = time.time(), self.step, 0.0
+        # held-out evaluation (--eval-data): at the boundary before every step that is a multiple of --eval-every, and
+        # once after the last step.  A boundary's evaluation is done once it has completed.  Every (re-)bind to a new
+        # generation forgets that (last_eval_step = -1): a joiner knows nothing of it, so after a rescale or a recovery at
+        # a boundary that was already evaluated -- a peer lost in the step right after an evaluation -- every rank of the
+        # new generation evaluates it again, and all of them issue the same collectives.
+        self.evals: List[Dict[str, Any]] = []
+        self.last_eval_step = -1
+
+    def _join_job(self) -> None:
+        """Join the job's process group and take its state, and with it the loop step to start at."""
+        args, adapter, rank = self.args, self.adapter, self.rank
+        joiner = bool(args.elastic and self.watcher is not None and self.generation > 1 and self.world > 1)
+        if joiner:
+            # Joining a running job: do everything that needs no peer first -- CUDA context, model build, two throw-away
+            # steps (kernel loading, cuDNN plans, allocator growth; the state is overwritten by rank 0's broadcast
+            # anyway) -- and only then tell the survivors, who keep training until this rank is ready to rendezvous.
+            adapter.bind(None, warm_up=True)     # single-micro-batch steps: not 2k micro-batches of throw-away work
+            for _ in range(2):
+                adapter.train_step()
+            if self.use_cuda:
+                torch.cuda.synchronize()
+            t = self.trace
+            t["prewarmed"] = time.time()
+            self.watcher.announce_ready(rank, self.generation)
+            self._log(f"joiner ready for generation {self.generation} after {t['prewarmed'] - t['process_start']:.2f}s "
+                      f"of local set-up (model build {t['model_built'] - t['process_start']:.2f}s, warm-up steps "
+                      f"{t['prewarmed'] - t['model_built']:.2f}s)")
+        if self.world > 1:
+            self._rendezvous()
+            if self.watcher is not None:
+                self.watcher.adopted(self.generation, self.world)
+        self.trace["rendezvous_done"] = time.time()
+        heartbeat(force=True)
+        adapter.bind(None)
+        self._log(f"world {self.world}: gradient sync = {adapter.gradient_sync}")
+        restart_count = env_int("TRAININGJOB_REPLICA_RESTARTCOUNT", 0)
+        start_step = 0
+        if restart_count > 0 and args.ckpt_every > 0:
+            start_step = load_checkpoint(args, adapter)
+            adapter.step_count = start_step
+            self._log(f"restart #{restart_count}: resumed from checkpoint at step {start_step}"
+                      + (f", data position {adapter.data_position}" if hasattr(adapter, "data_position") else ""))
+        # a joiner without a checkpoint only has its throw-away warm-up state: it must never be elected as the source
+        self.step = sync_state(adapter, start_step, self.device, have_state=not joiner or start_step > 0)
+        if joiner:
+            self._log(f"joined generation {self.generation} (world {self.world}) at step {self.step}")
+
+    def _log(self, message: str) -> None:
+        print(f"[worker {self.rank}] {message}", flush=True)
+
+    def _leave(self, message: str) -> None:
+        self._log(message)
+        raise _Left({"left": True, "generation": self.generation, "step": self.step})
+
+    def _rendezvous(self) -> None:
+        """Form the group of generation ``self.generation`` -- or of a newer one the job has moved on to meanwhile."""
+        got = rendezvous(self.rank, {"generation": self.generation, "world": self.world, "port": self.port}, self.device,
+                         self.watcher)
+        if got is None:
+            self._leave("not part of the current world any more, leaving")
+        self.generation, self.world, self.port = got["generation"], got["world"], got["port"]
+
+    def _enter(self, target: Dict[str, Any], t0: float, observed_at: float, recovered_from: Optional[str] = None,
+               aborted: bool = False) -> None:
+        """Move to rendezvous generation ``target`` once the old group is gone: rendezvous, re-bind the trainer, hand the
+        state off; the change is timed until the first step at the new world size completes (``_rescaled``).  A rank
+        outside the new world leaves.  A failed hand-off raises after a rescale, so the loop's recovery takes it over."""
+        self.generation, self.world, self.port = target["generation"], target["world"], target["port"]
+        if self.rank >= self.world:
+            self._leave(f"leaving: world shrinks to {self.world} (generation {self.generation})")
+        t1 = time.time()
+        if self.world > 1 or recovered_from is not None:    # a recovery re-reads the job even for a world of one
+            self._rendezvous()
+        t2 = time.time()
+        if aborted and self.args.ckpt_every > 0 and os.path.exists(ckpt_path(self.args)):
+            # kernels released by an abort ran on with whatever the dead peer left in the buffers: do not trust this
+            # rank's copy when there is a checkpoint to fall back to
+            self.step = load_checkpoint(self.args, self.adapter)
+            self.adapter.step_count = self.step
+        if self.breaker is not None:
+            self.breaker.tripped = False
+            self.breaker.progress(self.generation)
+        self.adapter.bind(None)
+        self.last_eval_step = -1
         try:
+            with guarded(self.breaker, "the state hand-off", self.generation):
+                self.step = sync_state(self.adapter, self.step, self.device)
+        except RuntimeError as e:
+            if recovered_from is None:
+                raise
+            # the hand-off is a chain of collectives on the new group: ANOTHER peer died under it.  The group is gone
+            # again; the step boundary's generation agreement finds the newest record and joins it through a rescale.
+            self._log(f"another peer was lost during the state hand-off of generation {self.generation} "
+                      f"({type(e).__name__}); joining the next generation")
+            teardown_group(broken=True)
+            if self.breaker is not None:
+                self.breaker.tripped = False
+            return
+        heartbeat(force=True)
+        self.watcher.adopted(self.generation, self.world)
+        self.pending_rescale = {"generation": self.generation, "world": self.world, "t0": t0, "observed_at": observed_at,
+                                "teardown_s": t1 - t0, "init_pg_s": t2 - t1, "sync_state_s": time.time() - t2}
+        if recovered_from is not None:
+            self.pending_rescale["recovered_from"] = recovered_from
+
+    def _rescale(self) -> bool:
+        """Elastic: agree on the newest rendezvous generation at the step boundary and move to it (True)."""
+        if self.watcher is None or not self.args.elastic:
+            return False
+        target = self.watcher.agree(self.device, guard=self.breaker)
+        if target is None or target["generation"] == self.generation:
+            return False
+        t0 = time.time()
+        self._log(f"rendezvous generation {self.generation} -> {target['generation']} "
+                  f"(world {self.world} -> {target['world']}) at step {self.step}")
+        if dist.is_initialized():
+            self.adapter.prepare_state()       # sharded optimizer state -> whole state on every survivor
+            if self.use_cuda:
+                torch.cuda.synchronize()
             dist.destroy_process_group()
-        except Exception:  # noqa: BLE001
-            pass
-    return result
+        self._enter(target, t0, target.get("observed_at", t0))
+        return True
+
+    def _recover(self, failure) -> None:
+        """faultTolerant: a peer died under a collective.  (gloo raises in the survivors; for NCCL the StallBreaker aborts
+        the communicator.)  The survivors keep their process, device state and -- on GPUs -- CUDA context: drop the
+        broken group, wait for the controller to replace the lost replica (restart scope Pod, new rendezvous
+        generation), re-rendezvous and continue from the survivors' state."""
+        t0 = time.time()
+        aborted = self.breaker is not None and self.breaker.tripped
+        self._log(f"step {self.step}: lost a peer ({failure[0]}: {failure[1]}); keeping state, waiting for the next "
+                  f"rendezvous generation")
+        # pending work handles keep the group's sockets open; a peer that is blocked on *us* (gloo does not
+        # propagate a failure beyond the dead rank's direct neighbours) only errors out once they really close
+        self.adapter.discard_step()
+        teardown_group(broken=True)
+        gc.collect()
+        target = wait_for_newer_generation(self.watcher, self.generation, float(os.environ.get("AITJ_FT_WAIT", "120")),
+                                           should_stop=lambda: self.stopping)
+        if target is None and self.stopping:
+            self._log("terminated while waiting for the job to be repaired")
+            return
+        if target is None:
+            self._log("no new rendezvous generation was published: giving up")
+            raise RuntimeError(f"collective failed and the job was not repaired: {failure[0]}: {failure[1]}")
+        self._enter(target, t0, t0, recovered_from=failure[0], aborted=aborted)
+
+    def _eval_due(self) -> bool:
+        s, a = self.step, self.args
+        return hasattr(self.adapter, "eval_data") and s != self.last_eval_step and \
+            ((s > 0 and a.eval_every > 0 and s % a.eval_every == 0) or (a.steps > 0 and s >= self.total))
+
+    def _evaluate(self) -> None:
+        t_eval = time.perf_counter()
+        launches_before = oplib.LAUNCHES
+        if self.use_cuda:
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+        with guarded(self.breaker, "an evaluation", self.generation):
+            # an evaluation is as long as its micro-batches make it: the stall breaker sees progress after each one,
+            # not the patience of a single training step for the whole of it
+            rec = self.adapter.evaluate(
+                progress=None if self.breaker is None else lambda: self.breaker.progress(self.generation))
+        wall_ms = (time.perf_counter() - t_eval) * 1e3
+        if self.use_cuda:
+            e1.record()
+            e1.synchronize()
+        ms = e0.elapsed_time(e1) if self.use_cuda else wall_ms
+        self.region.exclude(ms, wall_ms, oplib.LAUNCHES - launches_before)
+        self.live_eval_s += wall_ms / 1e3
+        rec = {"step": self.step, "loss": rec["loss"], "tokens": rec["tokens"], "samples": rec["samples"],
+               "ms": round(ms, 3)}
+        self.evals.append(rec)
+        self.last_eval_step = self.step
+        if self.rank == 0:
+            self._log(f"step {self.step}: eval loss {rec['loss']:.6f} over {rec['samples']} held-out windows "
+                      f"({rec['tokens']} tokens) in {ms:.1f} ms")
+
+    def run(self) -> Dict[str, Any]:
+        while (self.step < self.total or self._eval_due()) and not self.stopping:
+            if self.breaker is not None:
+                self.breaker.progress(self.generation)
+                # patience from this generation's completed steps: the first step on a freshly bound trainer captures
+                # CUDA graphs / loads kernels, and an accumulated step can take seconds -- neither is a stall
+                self.breaker.begin_step(self.generation)
+            failure = None
+            try:
+                if self._rescale():
+                    continue    # back to the step boundary: every rank (joiners included) runs the same sequence
+                if self.region.from_step < 0 and self.step >= self.args.warmup and self.args.steps > 0:
+                    self.region.arm(self.step, self.world)
+                if self._eval_due():
+                    self._evaluate()
+                    if self.step >= self.total:
+                        continue          # the evaluation after the last step: the loop ends here
+                with guarded(self.breaker, "this step", self.generation):
+                    t_step = time.perf_counter()
+                    loss = self.adapter.train_step()
+                    if self.breaker is not None:
+                        self.breaker.step_done(self.generation, time.perf_counter() - t_step)
+            except RuntimeError as e:
+                # Without faultTolerant the error ends this replica and the job's restartPolicy / restartScope take
+                # over, as in the reference (pod.go:208-250).
+                if not self.fault_tolerant or self.world <= 1:
+                    raise
+                failure = (type(e).__name__, (str(e).splitlines() or [""])[0][:160])
+            if failure is not None:
+                # (outside the except block: the traceback of the failed step references the work handles of the broken
+                # group, and with them its sockets)
+                self._recover(failure)
+                continue
+            self._step_done(loss)
+        return self._finish()
+
+    def _step_done(self, loss: float) -> None:
+        self.losses.append(loss)
+        self.step += 1
+        heartbeat()
+        if self.pending_rescale is not None:
+            self._rescaled()
+        if "first_step_done" not in self.trace:
+            self.trace["first_step_done"] = time.time()
+            if self.watcher is not None:
+                self.watcher.report_trace(self.rank, self.trace)
+        if self.rank == 0 and self.watcher is not None and self.report_every > 0 and \
+                time.time() - self.live_t0 >= self.report_every:
+            self._report_live()
+        if self.args.ckpt_every > 0 and self.step % self.args.ckpt_every == 0:
+            self.adapter.prepare_state()
+            if self.rank == 0:
+                save_checkpoint(self.args, self.adapter, self.adapter.step_count)
+        if self.args.step_sleep > 0:
+            time.sleep(self.args.step_sleep)
+
+    def _rescaled(self) -> None:
+        """The first completed step at the new world size ends the rescale."""
+        p, now = self.pending_rescale, time.time()
+        rec = {"generation": p["generation"], "world": p["world"], "seconds": now - p["t0"],
+               "since_change": now - p["observed_at"], "teardown_s": round(p["teardown_s"], 4),
+               "init_pg_s": round(p["init_pg_s"], 4), "sync_state_s": round(p["sync_state_s"], 4)}
+        rec["first_step_s"] = round(rec["seconds"] - rec["teardown_s"] - rec["init_pg_s"] - rec["sync_state_s"], 4)
+        if "recovered_from" in p:
+            rec["recovered_from"] = p["recovered_from"]
+            self.recoveries.append(rec)
+        self.rescales.append(rec)
+        self._log(f"step {self.step}: rescaled to world={rec['world']} gen={rec['generation']} in {rec['seconds']:.3f}s")
+        if self.watcher is not None:
+            self.watcher.report_rescale(self.rank, rec, force="recovered_from" in rec)   # rank 0 may be the replaced one
+        self.pending_rescale = None
+
+    def _report_live(self) -> None:
+        dt, n = time.time() - self.live_t0 - self.live_eval_s, self.step - self.live_step0
+        if n > 0 and dt > 0:
+            G = self.adapter.plan.global_batch
+            live = {"samples_per_sec": round(G * n / dt, 2), "ms_per_step": round(dt * 1e3 / n, 3), "world": self.world,
+                    "steps_done": self.step, "global_batch": G, "recoveries": len(self.recoveries)}
+            if self.evals:
+                live.update(eval_loss=self.evals[-1]["loss"], eval_step=self.evals[-1]["step"])
+            self.watcher.report_live(self.rank, live)
+        self.live_t0, self.live_step0, self.live_eval_s = time.time(), self.step, 0.0
+
+    def _finish(self) -> Dict[str, Any]:
+        args, adapter, losses, rank = self.args, self.adapter, self.losses, self.rank
+        result: Dict[str, Any] = {"rank": rank, "world": self.world, "steps_done": self.step,
+                                  "generation": self.generation, "final_loss": losses[-1] if losses else None,
+                                  "rescales": self.rescales, "recoveries": self.recoveries, "trace": self.trace}
+        if hasattr(adapter, "data_position"):
+            result["data_position"] = adapter.data_position
+        if hasattr(adapter, "eval_data"):
+            result.update(evals=self.evals, eval_loss_last=self.evals[-1]["loss"] if self.evals else None)
+        if self.breaker is not None:
+            self.breaker.stop()
+        if _CKPT.get("writer") is not None:
+            _CKPT["writer"].wait(60.0)
+        n_timed = self.step - self.region.from_step if self.region.from_step >= 0 else 0
+        if args.steps > 0 and self.step >= self.total and n_timed > 0:
+            plan = adapter.plan
+            result.update(self.region.close(self.step, self.world, self.device, plan.global_batch,
+                                            adapter.launches_per_step()))
+            result.update({
+                "global_batch": plan.global_batch, "batch_per_gpu": args.batch,
+                "micro_batches": plan.k, "micro_batches_this_rank": plan.n,
+                "h2d_bytes_per_step": adapter.h2d_bytes, "d2h_bytes_per_step": adapter.d2h_bytes,
+                "loss_first": losses[0] if losses else None, "loss_last": losses[-1] if losses else None,
+                "flops_per_step": getattr(adapter, "flops_per_step", 0.0) * plan.n,     # this rank's work
+                "describe": adapter.describe,
+            })
+            result.update(adapter.graph_report(self.world))
+        if args.dump_outputs and n_timed > 0:
+            # collective: with the owner-sharded optimizer each rank keeps only its own range of the master weights current
+            adapter.prepare_state()
+            if rank == 0:
+                dump_outputs(args.dump_outputs, adapter, losses[-n_timed:])
+        if rank == 0 and args.result:
+            os.makedirs(os.path.dirname(os.path.abspath(args.result)), exist_ok=True)
+            with open(args.result + ".tmp", "w") as f:
+                json.dump(result, f)
+            os.replace(args.result + ".tmp", args.result)
+        if rank == 0 and self.watcher is not None:
+            self.watcher.report_result(result)
+        if dist.is_initialized():
+            try:
+                dist.destroy_process_group()
+            except Exception:  # noqa: BLE001
+                pass
+        return result
+
+
+def run(args) -> Dict[str, Any]:
+    """One replica from start to end: the result record, or ``{"left": True, ...}`` when the job's world shrank
+    below this rank."""
+    try:
+        return _Loop(args).run()
+    except _Left as left:
+        return left.args[0]
 
 
 def parse_args(argv=None):
