@@ -130,11 +130,14 @@ class TransformerEngine:
                                                     os.environ.get("AITJ_WGRAD_STREAM", "0") != "0") else None
 
     # ------------------------------------------------------------------ GEMM front-ends
-    def _linear(self, x, w, out, bias=None, residual=None, gelu=False, aux=None):
+    def _linear(self, x, w, out, bias=None, residual=None, gelu=False, aux=None, block_n=None):
+        """out = x @ w^T (+ bias) (GELU, pre-activation to aux) (+ residual).  ``block_n``: the wgmma tile, None = the
+        engine's choice for this shape."""
         F = self.F
         if self.backend == "wgmma":
-            F.gemm(x, w, out, bias=bias, residual=residual, gelu=gelu, save_pre=gelu, aux=aux,
-                   block_n=self._bn(x.shape[0], w.shape[0], f"fwd:{w.shape[0]}x{w.shape[1]}"))
+            if block_n is None:
+                block_n = self._bn(x.shape[0], w.shape[0], f"fwd:{w.shape[0]}x{w.shape[1]}")
+            F.gemm(x, w, out, bias=bias, residual=residual, gelu=gelu, save_pre=gelu, aux=aux, block_n=block_n)
             return out
         # library path (cuBLAS) + standalone elementwise kernels; numerics cross-check / fallback bench arm
         y = torch.addmm(bias, x, w.t()) if bias is not None else x @ w.t()

@@ -392,3 +392,126 @@ def gelu_fwd(x, y):
 
 def gelu_bwd(x, dy, dx):
     lib.call("aitj_gelu_bwd", x.data_ptr(), dy.data_ptr(), dx.data_ptr(), x.numel(), _stream())
+
+
+# ------------------------------------------------------------------------------------ decoding (ops/csrc/decode.cu)
+# The decode entry points refuse nothing themselves: every argument is checked here, before the library is called.
+# ``check_*`` are the checks alone, so that stand-ins of these entry points can apply the same ones.
+DECODE_CHUNK = 64            # cache positions per attention_decode CTA
+SAMPLE_MAX_VOCAB = 102400    # sample_tokens stages a bf16 row of the vocabulary in shared memory (200 KB)
+
+
+def _need(ok: bool, msg: str) -> None:
+    if not ok:
+        raise ValueError(msg)
+
+
+def _tensor(t, name: str, dtype, ndim: int = None, align: int = 0) -> None:
+    _need(isinstance(t, torch.Tensor), f"{name} must be a tensor")
+    _need(t.dtype == dtype, f"{name} must be {dtype}, not {t.dtype}")
+    _need(t.is_contiguous(), f"{name} must be contiguous")
+    _need(ndim is None or t.dim() == ndim, f"{name} must have {ndim} dimensions, not {t.dim()}")
+    _need(not align or t.data_ptr() % align == 0, f"{name} must be {align}-byte aligned")
+
+
+def _check_pos(pos, n: int) -> None:
+    _tensor(pos, "pos", torch.int32)
+    _need(pos.numel() >= n, f"pos must hold at least {n} int32 elements")
+
+
+def decode_partials(S: int, H: int, Tmax: int) -> int:
+    """fp32 elements of ``attention_decode``'s scratch: (max, sum, 64 accumulators) per (sequence, head, key chunk)."""
+    return S * H * (-(-Tmax // DECODE_CHUNK)) * (64 + 2)
+
+
+def check_attention_decode(qkv, cache, pos, out, part, H: int):
+    """(S, Tmax) of a valid ``attention_decode`` call; ValueError otherwise."""
+    _tensor(qkv, "qkv", torch.bfloat16, 2, 16)
+    S = qkv.shape[0]
+    _need(S >= 1, "attention_decode needs S >= 1 sequences")
+    _need(H >= 1 and qkv.shape[1] == 3 * H * 64, f"qkv has {qkv.shape[1]} columns: H * 64 == C needs 3 * {H} * 64")
+    _tensor(cache, "cache", torch.bfloat16, 5, 16)
+    _need(cache.shape[0] == S and cache.shape[2:] == (2, H, 64),
+          f"cache must be [S={S}, Tmax, 2, H={H}, 64], not {tuple(cache.shape)}")
+    Tmax = cache.shape[1]
+    _need(Tmax >= 1, "cache must hold at least one position")
+    _tensor(out, "out", torch.bfloat16, 2, 16)
+    _need(tuple(out.shape) == (S, H * 64), f"out must be [{S}, {H * 64}], not {tuple(out.shape)}")
+    _tensor(part, "part", torch.float32)
+    _need(part.numel() >= decode_partials(S, H, Tmax), f"part must hold {decode_partials(S, H, Tmax)} fp32 elements")
+    _check_pos(pos, 1)
+    return S, Tmax
+
+
+def attention_decode(qkv, cache, pos, out, part, H: int):
+    """One decode step of one layer for S sequences at the shared position pos[0] (device int32 < Tmax): the new k and v
+    (columns C..3C of qkv bf16 [S, 3C], head dim 64) are written into cache bf16 [S, Tmax, 2, H, 64] at pos[0], and q
+    attends over positions [0, pos[0]] -> out bf16 [S, C].  ``part``: fp32 scratch of ``decode_partials`` elements."""
+    S, Tmax = check_attention_decode(qkv, cache, pos, out, part, H)
+    lib.call("aitj_attention_decode", qkv.data_ptr(), cache.data_ptr(), pos.data_ptr(), out.data_ptr(), part.data_ptr(),
+             S, H, Tmax, _stream())
+    lib.LAUNCHES += 1          # the merge of the key chunks rides along with the main kernel
+    return out
+
+
+def check_embedding_decode(tok, wte, wpe, pos, out) -> int:
+    """S of a valid ``embedding_decode`` call; ValueError otherwise."""
+    _tensor(tok, "tok", torch.int64, 1)
+    S = tok.numel()
+    _need(S >= 1, "embedding_decode needs S >= 1 sequences")
+    _tensor(wte, "wte", torch.bfloat16, 2, 16)
+    _tensor(wpe, "wpe", torch.bfloat16, 2, 16)
+    C = wte.shape[1]
+    _need(C % 8 == 0 and wpe.shape[1] == C, f"wte and wpe need the same width, a multiple of 8: {C}, {wpe.shape[1]}")
+    _tensor(out, "out", torch.bfloat16, 2, 16)
+    _need(tuple(out.shape) == (S, C), f"out must be [{S}, {C}], not {tuple(out.shape)}")
+    _check_pos(pos, 1)
+    return S
+
+
+def embedding_decode(tok, wte, wpe, pos, out):
+    """out[s] = wte[tok[s]] + wpe[pos[0]] (tok int64 [S], pos device int32)."""
+    S = check_embedding_decode(tok, wte, wpe, pos, out)
+    lib.call("aitj_embedding_decode", tok.data_ptr(), wte.data_ptr(), wpe.data_ptr(), pos.data_ptr(), out.data_ptr(),
+             S, wte.shape[1], _stream())
+    return out
+
+
+def check_sample_tokens(logits, vocab, tok, out_tokens, prompt, prompt_len, pos, temperature, top_k, seed,
+                        first_seq=0) -> int:
+    """S of a valid ``sample_tokens`` call; ValueError otherwise."""
+    _need(isinstance(logits, torch.Tensor) and logits.dtype == torch.bfloat16 and logits.dim() == 2,
+          "logits must be a 2-D bf16 tensor")
+    _need(logits.stride(1) == 1 and logits.stride(0) >= logits.shape[1], "logits rows must be contiguous")
+    S = logits.shape[0]
+    _need(S >= 1, "sample_tokens needs S >= 1 sequences")
+    _need(1 <= vocab <= logits.shape[1], f"vocab {vocab} must be in [1, {logits.shape[1]}] (the logits' columns)")
+    _need(vocab <= SAMPLE_MAX_VOCAB, f"vocab {vocab} exceeds {SAMPLE_MAX_VOCAB}: a row must fit in shared memory")
+    _tensor(tok, "tok", torch.int64, 1)
+    _need(tok.numel() == S, f"tok must hold {S} tokens, not {tok.numel()}")
+    _tensor(out_tokens, "out_tokens", torch.int64, 2)
+    _need(out_tokens.shape[0] == S, f"out_tokens must have {S} rows, not {out_tokens.shape[0]}")
+    _tensor(prompt, "prompt", torch.int64, 2)
+    _need(prompt.shape[0] == S, f"prompt must have {S} rows, not {prompt.shape[0]}")
+    _need(1 <= prompt_len <= prompt.shape[1], f"prompt_len {prompt_len} must be in [1, {prompt.shape[1]}]")
+    _check_pos(pos, 2)
+    _need(temperature >= 0 and temperature < float("inf"), f"temperature must be finite and >= 0, not {temperature}")
+    _need(0 <= top_k <= vocab, f"top_k must be in [0, vocab={vocab}], not {top_k}")
+    _need(0 <= seed < 1 << 63, f"seed must be in [0, 2^63), not {seed}")
+    _need(0 <= first_seq and first_seq + S <= 1 << 31, f"first_seq {first_seq} out of range")
+    return S
+
+
+def sample_tokens(logits, vocab, tok, out_tokens, prompt, prompt_len, pos, temperature, top_k, seed, first_seq=0):
+    """The next token of each sequence from its logits row (bf16 [S, Vp], columns >= ``vocab`` never chosen), at the shared
+    position p = pos[0]: the prompt's token prompt[s, p + 1] while p + 1 < prompt_len; else the argmax (lowest index on
+    ties) when ``temperature`` is 0 or ``top_k`` is 1; else one draw from softmax(logits / temperature) over the ``top_k``
+    largest logits (0 = all; ties with the top_k-th are kept), keyed by a Philox counter of (seed, first_seq + s, p), so
+    a sequence's tokens never depend on S or its row.  Writes tok[s] and out_tokens[s, p + 1] (when in range), then moves
+    pos[0] to p + 1; pos[1] is the kernel's completion count and must be 0 (it is 0 again afterwards)."""
+    S = check_sample_tokens(logits, vocab, tok, out_tokens, prompt, prompt_len, pos, temperature, top_k, seed,
+                            first_seq)
+    lib.call("aitj_sample_tokens", logits.data_ptr(), logits.stride(0), int(vocab), tok.data_ptr(),
+             out_tokens.data_ptr(), out_tokens.shape[1], prompt.data_ptr(), prompt.shape[1], int(prompt_len),
+             pos.data_ptr(), float(temperature), int(top_k), int(seed), int(first_seq), S, _stream())
+    return tok

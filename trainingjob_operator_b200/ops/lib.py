@@ -88,6 +88,9 @@ _SIGS = {
     "aitj_fused_set_peers": [_P, _P, _P, _I],
     "aitj_gelu_fwd": [_P, _P, _L, _P],
     "aitj_gelu_bwd": [_P, _P, _P, _L, _P],
+    "aitj_attention_decode": [_P, _P, _P, _P, _P, _I, _I, _I, _P],
+    "aitj_embedding_decode": [_P, _P, _P, _P, _P, _I, _I, _P],
+    "aitj_sample_tokens": [_P, _I, _I, _P, _P, _I, _P, _I, _I, _P, _F, _I, _L, _I, _I, _P],
 }
 
 

@@ -88,6 +88,18 @@ class EngineAdapter:
                 if self.eval_samples > self.eval_data.n_windows:
                     raise DataError(f"--eval-samples {self.eval_samples}: --eval-data {args.eval_data!r} holds only "
                                     f"{self.eval_data.n_windows} windows of {seq + 1} tokens")
+            if getattr(args, "generate_every", None) is not None:
+                # text generation at step boundaries: a generator of its own (buffers, KV caches) on the engine's
+                # weights, built at the first generation
+                self.generator = None
+                self.tokenizer = None
+                if args.tokenizer:
+                    from .tokenizer import Tokenizer, TokenizerError
+
+                    self.tokenizer = Tokenizer(args.tokenizer)
+                    if self.tokenizer.vocab_size < cfg.vocab_size:
+                        raise TokenizerError(f"{args.tokenizer}: {self.tokenizer.vocab_size} tokens, fewer than the "
+                                             f"{cfg.vocab_size} of {cfg.name}")
         self.cfg = cfg
         self.batch, self.seq = batch, seq
         self.h2d_bytes = self.data.bytes_per_sample * batch if hasattr(self, "data_position") else \
@@ -173,6 +185,30 @@ class EngineAdapter:
         called after each of this rank's micro-batches is enqueued."""
         total, tokens = self.trainer.evaluate(self._eval_inputs(progress))
         return {"loss": total / max(1, tokens), "tokens": tokens, "samples": self.eval_samples}
+
+    def generate(self, step: int, progress=None) -> Dict[str, Any]:
+        """``--generate-count`` sequences of the prompt and ``--generate-tokens`` new tokens, sampled with the seed of this
+        step (``generation_seed``).  Local: every rank computes the same from its own copy of the weights.  ``progress``
+        is called every few tokens."""
+        from ..models.generate import GPT2Generator, generation_seed
+
+        a = self.args
+        if self.generator is None:
+            self.generator = GPT2Generator(self.engine, a.generate_count, len(a.generate_prompt) + a.generate_tokens)
+        seed = generation_seed(a.seed, step)
+
+        def tick(_tokens):
+            heartbeat()
+            if progress is not None:
+                progress()
+
+        toks = self.generator.generate(a.generate_prompt, a.generate_tokens, temperature=a.temperature, top_k=a.top_k,
+                                       seed=seed, use_graph=not a.no_graph and self.engine.dev.type == "cuda",
+                                       progress=tick)
+        rec: Dict[str, Any] = {"seed": seed, "tokens": toks.tolist()}
+        if self.tokenizer is not None:
+            rec["text"] = [self.tokenizer.decode(t) for t in rec["tokens"]]
+        return rec
 
     def discard_step(self) -> None:
         self.engine.params.g32.zero_()
@@ -509,7 +545,7 @@ class _TimedRegion:
         self.launches0 = oplib.LAUNCHES
 
     def exclude(self, ms: float, wall_ms: float, launches: int) -> None:
-        """An evaluation ran: out of the step figures if it was inside the region."""
+        """An evaluation or a generation ran: out of the step figures if it was inside the region."""
         if self.from_step >= 0:
             self.eval_ms += ms
             self.eval_wall_ms += wall_ms
@@ -600,6 +636,10 @@ class _Loop:
         # new generation evaluates it again, and all of them issue the same collectives.
         self.evals: List[Dict[str, Any]] = []
         self.last_eval_step = -1
+        # text generation (--generate-every): at the same boundaries, after the evaluation; local to each rank, so a
+        # boundary is generated once per process whatever happens to the group around it
+        self.generations: List[Dict[str, Any]] = []
+        self.last_generate_step = -1
 
     def _join_job(self) -> None:
         """Join the job's process group and take its state, and with it the loop step to start at."""
@@ -745,24 +785,47 @@ class _Loop:
         return hasattr(self.adapter, "eval_data") and s != self.last_eval_step and \
             ((s > 0 and a.eval_every > 0 and s % a.eval_every == 0) or (a.steps > 0 and s >= self.total))
 
-    def _evaluate(self) -> None:
-        t_eval = time.perf_counter()
+    def _off_the_clock(self, what: str, work):
+        """Run ``work(progress)`` -- an evaluation or a generation -- under the stall breaker, and take its device time,
+        wall time and kernel launches out of the step figures.  Returns (its result, device ms)."""
+        t0 = time.perf_counter()
         launches_before = oplib.LAUNCHES
         if self.use_cuda:
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             e0.record()
-        with guarded(self.breaker, "an evaluation", self.generation):
-            # an evaluation is as long as its micro-batches make it: the stall breaker sees progress after each one,
-            # not the patience of a single training step for the whole of it
-            rec = self.adapter.evaluate(
-                progress=None if self.breaker is None else lambda: self.breaker.progress(self.generation))
-        wall_ms = (time.perf_counter() - t_eval) * 1e3
+        with guarded(self.breaker, what, self.generation):
+            # as long as its pieces make it: the stall breaker sees progress after each one, not the patience of a
+            # single training step for the whole of it
+            out = work(None if self.breaker is None else lambda: self.breaker.progress(self.generation))
+        wall_ms = (time.perf_counter() - t0) * 1e3
         if self.use_cuda:
             e1.record()
             e1.synchronize()
         ms = e0.elapsed_time(e1) if self.use_cuda else wall_ms
         self.region.exclude(ms, wall_ms, oplib.LAUNCHES - launches_before)
         self.live_eval_s += wall_ms / 1e3
+        return out, ms
+
+    def _generate_due(self) -> bool:
+        s, a = self.step, self.args
+        every = getattr(a, "generate_every", None)
+        return every is not None and hasattr(self.adapter, "generator") and s != self.last_generate_step and \
+            ((s > 0 and every > 0 and s % every == 0) or (a.steps > 0 and s >= self.total))
+
+    def _generate(self) -> None:
+        rec, ms = self._off_the_clock("a generation", lambda progress: self.adapter.generate(self.step, progress))
+        rec = dict(step=self.step, ms=round(ms, 3), **rec)
+        self.generations.append(rec)
+        self.last_generate_step = self.step
+        if self.rank == 0:
+            self._log(f"step {self.step}: generated {len(rec['tokens'])} sequences of {len(rec['tokens'][0])} tokens "
+                      f"in {ms:.1f} ms (seed {rec['seed']})")
+            for i, seq in enumerate(rec.get("text") or rec["tokens"]):
+                self._log(f"step {self.step}: generation {i}: {seq!r}" if "text" in rec else
+                          f"step {self.step}: generation {i}: {' '.join(map(str, seq))}")
+
+    def _evaluate(self) -> None:
+        rec, ms = self._off_the_clock("an evaluation", lambda progress: self.adapter.evaluate(progress=progress))
         rec = {"step": self.step, "loss": rec["loss"], "tokens": rec["tokens"], "samples": rec["samples"],
                "ms": round(ms, 3)}
         self.evals.append(rec)
@@ -772,7 +835,7 @@ class _Loop:
                       f"({rec['tokens']} tokens) in {ms:.1f} ms")
 
     def run(self) -> Dict[str, Any]:
-        while (self.step < self.total or self._eval_due()) and not self.stopping:
+        while (self.step < self.total or self._eval_due() or self._generate_due()) and not self.stopping:
             if self.breaker is not None:
                 self.breaker.progress(self.generation)
                 # patience from this generation's completed steps: the first step on a freshly bound trainer captures
@@ -786,8 +849,10 @@ class _Loop:
                     self.region.arm(self.step, self.world)
                 if self._eval_due():
                     self._evaluate()
-                    if self.step >= self.total:
-                        continue          # the evaluation after the last step: the loop ends here
+                if self._generate_due():
+                    self._generate()
+                if self.step >= self.total:
+                    continue              # the evaluation / generation after the last step: the loop ends here
                 with guarded(self.breaker, "this step", self.generation):
                     t_step = time.perf_counter()
                     loss = self.adapter.train_step()
@@ -863,6 +928,8 @@ class _Loop:
             result["data_position"] = adapter.data_position
         if hasattr(adapter, "eval_data"):
             result.update(evals=self.evals, eval_loss_last=self.evals[-1]["loss"] if self.evals else None)
+        if hasattr(adapter, "generator"):
+            result["generations"] = self.generations
         if self.breaker is not None:
             self.breaker.stop()
         if _CKPT.get("writer") is not None:
@@ -946,7 +1013,20 @@ def parse_args(argv=None):
     ap.add_argument("--eval-every", type=int, default=0, metavar="N",
                     help="evaluate before every step that is a multiple of N, and after the last step (0 = only after "
                          "the last step)")
+    # text generation (GPT-2): "generate", because "samples" already names data windows here
+    ap.add_argument("--generate-every", type=int, default=None, metavar="N",
+                    help="generate text before every step that is a multiple of N, and after the last step (0 = only "
+                         "after the last step)")
+    ap.add_argument("--generate-count", type=int, default=None, metavar="S", help="sequences per generation (4)")
+    ap.add_argument("--generate-tokens", type=int, default=None, metavar="K", help="new tokens per sequence (64)")
+    ap.add_argument("--generate-prompt", default=None, metavar="IDS",
+                    help="comma-separated prompt token ids (default: --eot-token)")
+    ap.add_argument("--temperature", type=float, default=None, help="sampling temperature, 0 = greedy (1.0)")
+    ap.add_argument("--top-k", type=int, default=None, help="sample among the K most likely tokens (0 = all)")
+    ap.add_argument("--tokenizer", default=None, metavar="PATH",
+                    help="an llm.c gpt2_tokenizer.bin: generations are also reported as text")
     args = ap.parse_args(argv)
+    _check_generation_args(ap, args)
     if args.eval_data and args.model not in ("gpt2", "gpt2-tiny"):
         ap.error(f"--eval-data evaluates GPT-2 models only, not {args.model}")
     if args.eval_data and args.gemm != "wgmma":
@@ -971,6 +1051,48 @@ def parse_args(argv=None):
         if args.doc_mask and not 0 <= args.eot_token < vocab:
             ap.error(f"--eot-token {args.eot_token} is outside the vocabulary of {args.model} (size {vocab})")
     return args
+
+
+def _check_generation_args(ap, args) -> None:
+    """Refuse generation flags that cannot run, and fill in the defaults of the others."""
+    given = [f for f, v in (("--generate-count", args.generate_count), ("--generate-tokens", args.generate_tokens),
+                            ("--generate-prompt", args.generate_prompt), ("--temperature", args.temperature),
+                            ("--top-k", args.top_k), ("--tokenizer", args.tokenizer)) if v is not None]
+    if args.generate_every is None:
+        if given:
+            ap.error(f"{', '.join(given)} need --generate-every")
+        return
+    if args.model not in ("gpt2", "gpt2-tiny"):
+        ap.error(f"--generate-every generates from GPT-2 models only, not {args.model}")
+    args.generate_count = 4 if args.generate_count is None else args.generate_count
+    args.generate_tokens = 64 if args.generate_tokens is None else args.generate_tokens
+    args.temperature = 1.0 if args.temperature is None else args.temperature
+    args.top_k = 0 if args.top_k is None else args.top_k
+    if args.generate_every < 0 or args.generate_tokens < 0 or args.top_k < 0 or not args.temperature >= 0:
+        ap.error("--generate-every, --generate-tokens, --temperature and --top-k cannot be negative")
+    if args.generate_count < 1:
+        ap.error(f"--generate-count {args.generate_count}: generate at least one sequence")
+    from ..models.gpt2 import GPT2Config
+
+    cfg = GPT2Config.small() if args.model == "gpt2" else GPT2Config.tiny()
+    if args.generate_prompt is None:
+        prompt = [args.eot_token]
+        what = f"the default prompt, --eot-token {args.eot_token},"
+    else:
+        try:
+            prompt = [int(t) for t in args.generate_prompt.split(",")]
+        except ValueError:
+            ap.error(f"--generate-prompt {args.generate_prompt!r} is not a comma-separated list of token ids")
+        what = "--generate-prompt id"
+    bad = [t for t in prompt if not 0 <= t < cfg.vocab_size]
+    if bad:
+        ap.error(f"{what} {bad[0]} is outside the vocabulary of {args.model} (size {cfg.vocab_size})")
+    args.generate_prompt = prompt
+    if args.top_k > cfg.vocab_size:
+        ap.error(f"--top-k {args.top_k} exceeds the vocabulary of {args.model} (size {cfg.vocab_size})")
+    if len(prompt) + args.generate_tokens > cfg.block_size:
+        ap.error(f"the prompt ({len(prompt)} tokens) plus --generate-tokens {args.generate_tokens} exceed the block size "
+                 f"of {args.model} ({cfg.block_size})")
 
 
 def main(argv=None) -> int:
