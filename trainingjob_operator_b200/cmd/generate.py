@@ -15,10 +15,12 @@ import sys
 
 import torch
 
+from ..models.gpt2 import GPT2_MODELS
+
 
 def parse_args(argv=None):
     ap = argparse.ArgumentParser(prog="aitj-generate")
-    ap.add_argument("--model", default="gpt2", choices=["gpt2", "gpt2-tiny"])
+    ap.add_argument("--model", default="gpt2", choices=list(GPT2_MODELS))
     ap.add_argument("--ckpt", required=True, metavar="PATH", help="a worker checkpoint (--ckpt-dir)")
     ap.add_argument("--prompt", default=None, metavar="IDS", help="comma-separated token ids (default: --eot-token)")
     ap.add_argument("--eot-token", type=int, default=50256)
@@ -43,12 +45,12 @@ def parse_args(argv=None):
 
 def main(argv=None, out=None) -> int:
     from ..models.generate import GPT2Generator
-    from ..models.gpt2 import GPT2Config, GPT2Engine
+    from ..models.gpt2 import GPT2Engine, gpt2_config
     from ..runtime.checkpoint import load_into
 
     args = parse_args(argv)
     out = out or sys.stdout
-    cfg = GPT2Config.small() if args.model == "gpt2" else GPT2Config.tiny()
+    cfg = gpt2_config(args.model)
     tokenizer = None
     if args.tokenizer:
         from ..runtime.tokenizer import Tokenizer

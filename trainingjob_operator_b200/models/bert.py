@@ -143,21 +143,21 @@ class BertEngine(TransformerEngine):
     def forward(self) -> torch.Tensor:
         F, P = self.F, self.params
         F.embedding3_fwd(self.tok, self.typ, P.w16("wte"), P.w16("wpe"), P.w16("wtt"), self.e0, self.T)
-        F.layernorm_fwd(self.e0, P.w16("emb_ln_w"), P.w16("emb_ln_b"), self.x0, self.e_mean, self.e_rstd)
+        self.layernorm_fwd(self.e0, P.w16("emb_ln_w"), P.w16("emb_ln_b"), self.x0, self.e_mean, self.e_rstd)
         x = self.x0
         for i, lb in enumerate(self.layers):
             p = f"h{i}."
             self._linear(x, P.w16(p + "qkv_w"), lb.qkv, bias=P.w16(p + "qkv_b"))
             self._attention_fwd(lb)
             self._linear(lb.att_in, P.w16(p + "proj_w"), lb.res1, bias=P.w16(p + "proj_b"), residual=x)
-            F.layernorm_fwd(lb.res1, P.w16(p + "ln1_w"), P.w16(p + "ln1_b"), lb.ln1, lb.ln1_mean, lb.ln1_rstd)      # y
+            self.layernorm_fwd(lb.res1, P.w16(p + "ln1_w"), P.w16(p + "ln1_b"), lb.ln1, lb.ln1_mean, lb.ln1_rstd)   # y
             self._linear(lb.ln1, P.w16(p + "fc_w"), lb.fc_act, bias=P.w16(p + "fc_b"), gelu=True, aux=lb.fc_pre)
             self._linear(lb.fc_act, P.w16(p + "fc2_w"), lb.res2, bias=P.w16(p + "fc2_b"), residual=lb.ln1)
-            F.layernorm_fwd(lb.res2, P.w16(p + "ln2_w"), P.w16(p + "ln2_b"), lb.ln2, lb.ln2_mean, lb.ln2_rstd)
+            self.layernorm_fwd(lb.res2, P.w16(p + "ln2_w"), P.w16(p + "ln2_b"), lb.ln2, lb.ln2_mean, lb.ln2_rstd)
             x = lb.ln2
         # MLM head: dense + GELU + LayerNorm, decoder tied to the word embeddings (+ its own bias)
         self._linear(x, P.w16("mlm_w"), self.mlm_act, bias=P.w16("mlm_b"), gelu=True, aux=self.mlm_pre)
-        F.layernorm_fwd(self.mlm_act, P.w16("mlm_ln_w"), P.w16("mlm_ln_b"), self.mlm_ln, self.m_mean, self.m_rstd)
+        self.layernorm_fwd(self.mlm_act, P.w16("mlm_ln_w"), P.w16("mlm_ln_b"), self.mlm_ln, self.m_mean, self.m_rstd)
         self._linear(self.mlm_ln, P.w16("wte"), self.logits, bias=P.w16("dec_b"))
         return self._loss(self.n_masked)
 
@@ -171,8 +171,8 @@ class BertEngine(TransformerEngine):
         F.colsum(dlogits, P.grad("dec_b"))
         self._dgrad(dlogits, P.w16("wte"), d_t)
         self._wgrad(dlogits, self.mlm_ln, P.grad("wte"))
-        F.layernorm_bwd(d_t, self.mlm_act, P.w16("mlm_ln_w"), self.m_mean, self.m_rstd, d_g, P.grad("mlm_ln_w"),
-                        P.grad("mlm_ln_b"))
+        self.layernorm_bwd(d_t, self.mlm_act, P.w16("mlm_ln_w"), self.m_mean, self.m_rstd, d_g, P.grad("mlm_ln_w"),
+                           P.grad("mlm_ln_b"))
         F.gelu_bwd(self.mlm_pre, d_g, d_u)
         F.colsum(d_u, P.grad("mlm_b"))
         self._wgrad(d_u, x_last, P.grad("mlm_w"))
@@ -191,16 +191,16 @@ class BertEngine(TransformerEngine):
         free = [t for t in self.d_x if t is not self._d_cur]
         d_r, d_y = free
         # x_{l+1} = LN2(y + MLP(y))
-        F.layernorm_bwd(self._d_cur, lb.res2, P.w16(p + "ln2_w"), lb.ln2_mean, lb.ln2_rstd, d_r, P.grad(p + "ln2_w"),
-                        P.grad(p + "ln2_b"), dxsum=P.grad(p + "fc2_b"))
+        self.layernorm_bwd(self._d_cur, lb.res2, P.w16(p + "ln2_w"), lb.ln2_mean, lb.ln2_rstd, d_r,
+                           P.grad(p + "ln2_w"), P.grad(p + "ln2_b"), dxsum=P.grad(p + "fc2_b"))
         e_fc2 = self._wgrad(d_r, lb.fc_act, P.grad(p + "fc2_w"))
         self._dgrad(d_r, P.w16(p + "fc2_w"), self.d_fc, dgelu_aux=lb.fc_pre, colsum=P.grad(p + "fc_b"))
         self._wgrad(self.d_fc, lb.ln1, P.grad(p + "fc_w"))
         self._dgrad(self.d_fc, P.w16(p + "fc_w"), d_y, residual=d_r)            # + the skip connection's gradient
         # y = LN1(x + Attn(x))
         d_r1 = self._d_cur                                                      # its content is no longer needed
-        F.layernorm_bwd(d_y, lb.res1, P.w16(p + "ln1_w"), lb.ln1_mean, lb.ln1_rstd, d_r1, P.grad(p + "ln1_w"),
-                        P.grad(p + "ln1_b"), dxsum=P.grad(p + "proj_b"))
+        self.layernorm_bwd(d_y, lb.res1, P.w16(p + "ln1_w"), lb.ln1_mean, lb.ln1_rstd, d_r1, P.grad(p + "ln1_w"),
+                           P.grad(p + "ln1_b"), dxsum=P.grad(p + "proj_b"))
         self._wgrad(d_r1, lb.att_in, P.grad(p + "proj_w"))
         self._dgrad(d_r1, P.w16(p + "proj_w"), self.d_att)
         self._attention_bwd(lb, self.d_att, self.d_qkv, P.grad(p + "qkv_b"))
@@ -219,8 +219,8 @@ class BertEngine(TransformerEngine):
         # of tests/kernel_emulation.py: h0.proj_w came out wrong with AITJ_WGRAD_STREAM=1)
         self._join_wgrads()
         d_e = next(t for t in self.d_x if t is not self._d_cur)
-        F.layernorm_bwd(self._d_cur, self.e0, P.w16("emb_ln_w"), self.e_mean, self.e_rstd, d_e, P.grad("emb_ln_w"),
-                        P.grad("emb_ln_b"))
+        self.layernorm_bwd(self._d_cur, self.e0, P.w16("emb_ln_w"), self.e_mean, self.e_rstd, d_e, P.grad("emb_ln_w"),
+                           P.grad("emb_ln_b"))
         F.embedding3_bwd(self.tok, self.typ, d_e, P.grad("wte"), P.grad("wpe"), P.grad("wtt"), self.T)
         P.push_small_grads()
         self._join_wgrads()

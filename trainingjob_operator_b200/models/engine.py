@@ -38,6 +38,10 @@ class _LayerBufs:
         self.lse = None              # [B, H, T] fp32, only with the wgmma attention forward
 
 
+# widths at which the engines run fused_ops.cu's LayerNorm pair; layernorm_wide.cu serves every other multiple of 8
+FUSED_LAYERNORM_WIDTHS = (256, 512, 768)
+
+
 class TransformerEngine:
     """Explicit fwd/bwd/optimizer for a fixed (B, T) micro-batch on one GPU.
 
@@ -50,7 +54,7 @@ class TransformerEngine:
                  causal: bool, doc_mask: bool):
         from ..ops import functional as F
 
-        assert seq_len <= cfg.block_size and cfg.n_embd % 256 == 0
+        assert seq_len <= cfg.block_size
         self.F = F
         self.cfg = cfg
         self.B, self.T = batch_size, seq_len
@@ -99,6 +103,17 @@ class TransformerEngine:
             raise ValueError(f"gemm_backend must be 'wgmma' or 'cublas', not {self.backend!r}")
         cfg, T = self.cfg, self.T
         head_dim = cfg.n_embd // cfg.n_head
+        # LayerNorm by width: fused_ops.cu's pair where it runs fastest (GPT-2 small, BERT-base); layernorm_wide.cu's
+        # for the widths that pair refuses (GPT-2 large 1280, XL 1600) and for 1024 (GPT-2 medium), where the fused
+        # backward spills and the wide pair measured faster (docs/gpt2_sizes_h100_700w.json)
+        C = cfg.n_embd
+        if C in FUSED_LAYERNORM_WIDTHS:
+            self.ln_impl = "fused"
+        elif C % 8 == 0 and 8 <= C <= self.F.LAYERNORM_WIDE_MAX_C:
+            self.ln_impl = "wide"
+        else:
+            raise ValueError(f"no LayerNorm kernel serves n_embd={C}: the widths served are multiples of 8 up to "
+                             f"{self.F.LAYERNORM_WIDE_MAX_C}")
         if self.doc_mask:
             why = [w for bad, w in ((not self.causal, "it needs causal attention"),
                                     (T % 128, f"the sequence length {T} is not a multiple of 128"),
@@ -128,6 +143,17 @@ class TransformerEngine:
         # weight-gradient GEMMs on a side stream (AITJ_WGRAD_STREAM=0: in line); see _wgrad
         self.wgrad_stream = torch.cuda.Stream() if (self.dev.type == "cuda" and self.backend == "wgmma" and
                                                     os.environ.get("AITJ_WGRAD_STREAM", "0") != "0") else None
+
+    # ------------------------------------------------------------------ LayerNorm front-ends
+    def layernorm_fwd(self, x, gamma, beta, y, mean, rstd):
+        """y = LayerNorm(x), with the per-row mean and rstd, on the kernel ``_choose_kernel_paths`` chose."""
+        fn = self.F.layernorm_fwd if self.ln_impl == "fused" else self.F.layernorm_wide_fwd
+        return fn(x, gamma, beta, y, mean, rstd)
+
+    def layernorm_bwd(self, dy, x, gamma, mean, rstd, dx, dgamma, dbeta, dres=None, dxsum=None):
+        """dx = LN'(dy) (+ dres); dgamma, dbeta and dxsum (the previous linear's bias gradient) accumulate."""
+        fn = self.F.layernorm_bwd if self.ln_impl == "fused" else self.F.layernorm_wide_bwd
+        return fn(dy, x, gamma, mean, rstd, dx, dgamma, dbeta, dres=dres, dxsum=dxsum)
 
     # ------------------------------------------------------------------ GEMM front-ends
     def _linear(self, x, w, out, bias=None, residual=None, gelu=False, aux=None, block_n=None):

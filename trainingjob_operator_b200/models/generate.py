@@ -79,15 +79,15 @@ class GPT2Generator:
         F.embedding_decode(b["tok"], P.w16("wte"), P.w16("wpe"), b["pos"], x)
         for i, cache in enumerate(self.caches):
             p = f"h{i}."
-            F.layernorm_fwd(x, P.w16(p + "ln1_w"), P.w16(p + "ln1_b"), ln, b["mean"], b["rstd"])
+            e.layernorm_fwd(x, P.w16(p + "ln1_w"), P.w16(p + "ln1_b"), ln, b["mean"], b["rstd"])
             e._linear(ln, P.w16(p + "qkv_w"), b["qkv"], bias=P.w16(p + "qkv_b"), block_n=bn)
             F.attention_decode(b["qkv"], cache, b["pos"], b["att"], b["part"], self.cfg.n_head)
             e._linear(b["att"], P.w16(p + "proj_w"), res1, bias=P.w16(p + "proj_b"), residual=x, block_n=bn)
-            F.layernorm_fwd(res1, P.w16(p + "ln2_w"), P.w16(p + "ln2_b"), ln, b["mean"], b["rstd"])
+            e.layernorm_fwd(res1, P.w16(p + "ln2_w"), P.w16(p + "ln2_b"), ln, b["mean"], b["rstd"])
             e._linear(ln, P.w16(p + "fc_w"), b["fc_act"], bias=P.w16(p + "fc_b"), gelu=True, aux=b["fc_pre"],
                       block_n=bn)
             e._linear(b["fc_act"], P.w16(p + "fc2_w"), x, bias=P.w16(p + "fc2_b"), residual=res1, block_n=bn)
-        F.layernorm_fwd(x, P.w16("lnf_w"), P.w16("lnf_b"), ln, b["mean"], b["rstd"])
+        e.layernorm_fwd(x, P.w16("lnf_w"), P.w16("lnf_b"), ln, b["mean"], b["rstd"])
         e._linear(ln, P.w16("wte"), b["logits"], block_n=bn)
         F.sample_tokens(b["logits"], self.cfg.vocab_size, b["tok"], b["out"], b["prompt"], prompt_len, b["pos"],
                         temperature, top_k, seed, first_seq)

@@ -13,6 +13,7 @@ step is captured in one CUDA graph.  Only scaled-dot-product attention calls a l
 """
 from __future__ import annotations
 
+import dataclasses
 import math
 from dataclasses import dataclass
 from typing import List, Tuple
@@ -44,6 +45,22 @@ class GPT2Config:
     @staticmethod
     def tiny() -> "GPT2Config":
         return GPT2Config(vocab_size=1000, n_layer=2, n_head=4, n_embd=256, block_size=128, name="gpt2-tiny")
+
+
+# The GPT-2 models by the name workers and ``cmd/generate`` take (``--model``).  Every size has head dim 64, vocabulary
+# 50257 (50304 padded) and block size 1024; ``gpt2-tiny`` is for tests.
+GPT2_MODELS = {
+    "gpt2": GPT2Config.small(),
+    "gpt2-medium": GPT2Config(n_layer=24, n_head=16, n_embd=1024, name="gpt2-medium"),
+    "gpt2-large": GPT2Config(n_layer=36, n_head=20, n_embd=1280, name="gpt2-large"),
+    "gpt2-xl": GPT2Config(n_layer=48, n_head=25, n_embd=1600, name="gpt2-xl"),
+    "gpt2-tiny": GPT2Config.tiny(),
+}
+
+
+def gpt2_config(name: str) -> GPT2Config:
+    """A copy of the ``GPT2_MODELS`` entry ``name``."""
+    return dataclasses.replace(GPT2_MODELS[name])
 
 
 def gpt2_param_specs(cfg: GPT2Config) -> List[ParamSpec]:
@@ -140,15 +157,15 @@ class GPT2Engine(TransformerEngine):
         x = self.x0
         for i, lb in enumerate(self.layers):
             p = f"h{i}."
-            F.layernorm_fwd(x, P.w16(p + "ln1_w"), P.w16(p + "ln1_b"), lb.ln1, lb.ln1_mean, lb.ln1_rstd)
+            self.layernorm_fwd(x, P.w16(p + "ln1_w"), P.w16(p + "ln1_b"), lb.ln1, lb.ln1_mean, lb.ln1_rstd)
             self._linear(lb.ln1, P.w16(p + "qkv_w"), lb.qkv, bias=P.w16(p + "qkv_b"))
             self._attention_fwd(lb)
             self._linear(lb.att_in, P.w16(p + "proj_w"), lb.res1, bias=P.w16(p + "proj_b"), residual=x)
-            F.layernorm_fwd(lb.res1, P.w16(p + "ln2_w"), P.w16(p + "ln2_b"), lb.ln2, lb.ln2_mean, lb.ln2_rstd)
+            self.layernorm_fwd(lb.res1, P.w16(p + "ln2_w"), P.w16(p + "ln2_b"), lb.ln2, lb.ln2_mean, lb.ln2_rstd)
             self._linear(lb.ln2, P.w16(p + "fc_w"), lb.fc_act, bias=P.w16(p + "fc_b"), gelu=True, aux=lb.fc_pre)
             self._linear(lb.fc_act, P.w16(p + "fc2_w"), lb.res2, bias=P.w16(p + "fc2_b"), residual=lb.res1)
             x = lb.res2
-        F.layernorm_fwd(x, P.w16("lnf_w"), P.w16("lnf_b"), self.lnf, self.lnf_mean, self.lnf_rstd)
+        self.layernorm_fwd(x, P.w16("lnf_w"), P.w16("lnf_b"), self.lnf, self.lnf_mean, self.lnf_rstd)
 
     @torch.no_grad()
     def _bwd_head(self) -> None:
@@ -159,8 +176,8 @@ class GPT2Engine(TransformerEngine):
         self._d_cur, self._d_spare = self.d_res
         x_last = self.layers[-1].res2 if self.layers else self.x0
         last = len(self.layers) - 1
-        F.layernorm_bwd(self.d_ln, x_last, P.w16("lnf_w"), self.lnf_mean, self.lnf_rstd, self._d_cur, P.grad("lnf_w"),
-                        P.grad("lnf_b"), dxsum=P.grad(f"h{last}.fc2_b") if last >= 0 else None)
+        self.layernorm_bwd(self.d_ln, x_last, P.w16("lnf_w"), self.lnf_mean, self.lnf_rstd, self._d_cur,
+                           P.grad("lnf_w"), P.grad("lnf_b"), dxsum=P.grad(f"h{last}.fc2_b") if last >= 0 else None)
         if self.segment_join:
             self._join_wgrads()
 
@@ -179,8 +196,8 @@ class GPT2Engine(TransformerEngine):
         self._dgrad(d_res, P.w16(p + "fc2_w"), self.d_fc, dgelu_aux=lb.fc_pre, colsum=P.grad(p + "fc_b"))
         self._wgrad(self.d_fc, lb.ln2, P.grad(p + "fc_w"))
         self._dgrad(self.d_fc, P.w16(p + "fc_w"), self.d_ln)
-        F.layernorm_bwd(self.d_ln, lb.res1, P.w16(p + "ln2_w"), lb.ln2_mean, lb.ln2_rstd, spare,
-                        P.grad(p + "ln2_w"), P.grad(p + "ln2_b"), dres=d_res, dxsum=P.grad(p + "proj_b"))
+        self.layernorm_bwd(self.d_ln, lb.res1, P.w16(p + "ln2_w"), lb.ln2_mean, lb.ln2_rstd, spare,
+                           P.grad(p + "ln2_w"), P.grad(p + "ln2_b"), dres=d_res, dxsum=P.grad(p + "proj_b"))
         d_res, spare = spare, d_res
         # attention
         self._wgrad(d_res, lb.att_in, P.grad(p + "proj_w"))
@@ -190,9 +207,9 @@ class GPT2Engine(TransformerEngine):
         self._dgrad(self.d_qkv, P.w16(p + "qkv_w"), self.d_ln)
         if e_fc2 is not None:
             torch.cuda.current_stream().wait_event(e_fc2)     # `spare` is the buffer the fc2 weight gradient read
-        F.layernorm_bwd(self.d_ln, x_in, P.w16(p + "ln1_w"), lb.ln1_mean, lb.ln1_rstd, spare,
-                        P.grad(p + "ln1_w"), P.grad(p + "ln1_b"), dres=d_res,
-                        dxsum=P.grad(f"h{i - 1}.fc2_b") if i > 0 else None)
+        self.layernorm_bwd(self.d_ln, x_in, P.w16(p + "ln1_w"), lb.ln1_mean, lb.ln1_rstd, spare,
+                           P.grad(p + "ln1_w"), P.grad(p + "ln1_b"), dres=d_res,
+                           dxsum=P.grad(f"h{i - 1}.fc2_b") if i > 0 else None)
         self._d_cur, self._d_spare = spare, d_res
         if self.segment_join:
             self._join_wgrads()

@@ -252,6 +252,78 @@ def layernorm_bwd(dy, x, gamma, mean, rstd, dx, dgamma, dbeta, dres=None, dxsum=
     return dx
 
 
+# ------------------------------------------------------------------------------------ wide LayerNorm (layernorm_wide.cu)
+# For the widths the pair above refuses, such as GPT-2 large (1280) and XL (1600): any C that is a multiple of 8, up to
+# LAYERNORM_WIDE_MAX_C.  Like the decode entry points, the library refuses nothing; every argument is checked here.
+LAYERNORM_WIDE_MAX_C = 2048
+
+
+def _check_rows(t, name: str, M: int, C: int) -> None:
+    _tensor(t, name, torch.bfloat16, 2, 16)
+    _need(tuple(t.shape) == (M, C), f"{name} must be [{M}, {C}], not {tuple(t.shape)}")
+
+
+def _check_wide_input(x, gamma, mean, rstd):
+    _tensor(x, "x", torch.bfloat16, 2, 16)
+    M, C = x.shape
+    _need(C % 8 == 0 and 8 <= C <= LAYERNORM_WIDE_MAX_C,
+          f"the wide LayerNorm needs a width that is a multiple of 8 in [8, {LAYERNORM_WIDE_MAX_C}], not {C}")
+    _tensor(gamma, "gamma", torch.bfloat16, 1, 8)
+    _need(gamma.numel() == C, f"gamma must hold {C} elements, not {gamma.numel()}")
+    for t, name in ((mean, "mean"), (rstd, "rstd")):
+        _tensor(t, name, torch.float32, 1)
+        _need(t.numel() == M, f"{name} must hold {M} elements, not {t.numel()}")
+    return M, C
+
+
+def check_layernorm_wide_fwd(x, gamma, beta, y, mean, rstd, eps=1e-5):
+    """(M, C) of a valid ``layernorm_wide_fwd`` call; ValueError otherwise."""
+    M, C = _check_wide_input(x, gamma, mean, rstd)
+    _tensor(beta, "beta", torch.bfloat16, 1, 8)
+    _need(beta.numel() == C, f"beta must hold {C} elements, not {beta.numel()}")
+    _check_rows(y, "y", M, C)
+    return M, C
+
+
+def layernorm_wide_fwd(x, gamma, beta, y, mean, rstd, eps=1e-5):
+    """``layernorm_fwd`` for any width that is a multiple of 8 up to ``LAYERNORM_WIDE_MAX_C``: y (bf16), and the fp32
+    per-row mean and rstd the backward reads."""
+    M, C = check_layernorm_wide_fwd(x, gamma, beta, y, mean, rstd, eps)
+    lib.call("aitj_layernorm_wide_fwd", x.data_ptr(), gamma.data_ptr(), beta.data_ptr(), y.data_ptr(), mean.data_ptr(),
+             rstd.data_ptr(), M, C, float(eps), _stream())
+    return y
+
+
+def check_layernorm_wide_bwd(dy, x, gamma, mean, rstd, dx, dgamma, dbeta, dres=None, dxsum=None):
+    """(M, C) of a valid ``layernorm_wide_bwd`` call; ValueError otherwise."""
+    M, C = _check_wide_input(x, gamma, mean, rstd)
+    _check_rows(dy, "dy", M, C)
+    _check_rows(dx, "dx", M, C)
+    if dres is not None:
+        _check_rows(dres, "dres", M, C)
+    mode = _is_mc(dgamma)
+    for t, name in ((dgamma, "dgamma"), (dbeta, "dbeta"), (dxsum, "dxsum")):
+        if t is None and name == "dxsum":
+            continue
+        _need(t is not None and t.dtype == torch.float32 and tuple(t.shape) == (C,),
+              f"{name} must be an fp32 gradient of shape ({C},)")
+        _need(not isinstance(t, torch.Tensor) or t.is_contiguous(), f"{name} must be contiguous")
+        _need(t.data_ptr() % 4 == 0, f"{name} must be 4-byte aligned")
+        _need(_is_mc(t) == mode, "dgamma, dbeta and dxsum must all be local, all multicast or all owner-sharded")
+    return M, C
+
+
+def layernorm_wide_bwd(dy, x, gamma, mean, rstd, dx, dgamma, dbeta, dres=None, dxsum=None):
+    """``layernorm_bwd`` for the widths of ``layernorm_wide_fwd``, with the same fusions: dx = LN'(dy) (+ dres) in bf16;
+    dgamma, dbeta and dxsum (optional: colsum(dx), the bias gradient of the linear layer that produced x) are added to
+    fp32 gradients, local, multicast or owner-sharded."""
+    M, C = check_layernorm_wide_bwd(dy, x, gamma, mean, rstd, dx, dgamma, dbeta, dres, dxsum)
+    lib.call("aitj_layernorm_wide_bwd", dy.data_ptr(), x.data_ptr(), gamma.data_ptr(), mean.data_ptr(),
+             rstd.data_ptr(), _ptr(dres), dx.data_ptr(), dgamma.data_ptr(), dbeta.data_ptr(), _ptr(dxsum), M, C,
+             _is_mc(dgamma), _stream())
+    return dx
+
+
 def embedding_fwd(tok, wte, wpe, out, T):
     M, C = out.shape
     lib.call("aitj_embedding_fwd", tok.data_ptr(), wte.data_ptr(), _ptr(wpe), out.data_ptr(), M, T, C, _stream())

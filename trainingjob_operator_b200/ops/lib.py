@@ -70,6 +70,8 @@ _SIGS = {
     "aitj_xent_finish": [_P, _P, _P, _P, _P, _I, _I, _P],
     "aitj_layernorm_fwd": [_P, _P, _P, _P, _P, _P, _I, _I, _F, _P],
     "aitj_layernorm_bwd": [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _P],
+    "aitj_layernorm_wide_fwd": [_P, _P, _P, _P, _P, _P, _I, _I, _F, _P],
+    "aitj_layernorm_wide_bwd": [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _P],
     "aitj_embedding_fwd": [_P, _P, _P, _P, _I, _I, _I, _P],
     "aitj_embedding_bwd": [_P, _P, _P, _P, _I, _I, _I, _I, _P],
     "aitj_embedding3_fwd": [_P, _P, _P, _P, _P, _P, _I, _I, _I, _P],

@@ -32,6 +32,7 @@ from typing import Any, Dict, List, Optional
 import torch
 import torch.distributed as dist
 
+from ..models.gpt2 import GPT2_MODELS
 from ..ops import lib as oplib
 from .elastic import ElasticWatcher, env_int, rendezvous_from_env
 from .rendezvous import (StaleGeneration, StallBreaker, guarded, heartbeat, init_process_group,  # noqa: F401
@@ -46,7 +47,7 @@ class EngineAdapter:
     def __init__(self, name: str, batch: int, seq: int, args, device: str = "cuda"):
         """``device``: always "cuda" in a worker (``build_adapter``); the CPU dry-run tests pass "cpu" together with
         emulated kernel entry points (tests/kernel_emulation.py) to execute the adapter's control flow."""
-        from ..models.gpt2 import GPT2Config, GPT2Engine, flops_per_token
+        from ..models.gpt2 import GPT2Engine, flops_per_token, gpt2_config
 
         if name in ("bert", "bert-tiny"):
             # the real thing: word + position + token-type embeddings, post-LN bidirectional encoder, MLM head and loss
@@ -58,12 +59,9 @@ class EngineAdapter:
             self.data = SyntheticMLM(cfg.vocab_size, batch, seq, n_batches=4, seed=args.seed + 1, pin=device != "cpu")
             self.flops_per_step = bert_flops_per_token(cfg, seq) * batch * seq
         else:
-            if name == "gpt2":
-                cfg = GPT2Config.small()
-            elif name == "gpt2-tiny":
-                cfg = GPT2Config.tiny()
-            else:
+            if name not in GPT2_MODELS:
                 raise ValueError(name)
+            cfg = gpt2_config(name)
             seq = min(seq, cfg.block_size)
             doc_mask = bool(getattr(args, "doc_mask", False))
             self.engine = GPT2Engine(cfg, batch, seq, device, seed=args.seed, gemm_backend=args.gemm, causal=True,
@@ -446,7 +444,7 @@ class TorchAdapter:
 
 
 def build_adapter(args, device: torch.device):
-    if args.model in ("gpt2", "gpt2-tiny", "bert", "bert-tiny"):
+    if args.model in (*GPT2_MODELS, "bert", "bert-tiny"):
         if device.type != "cuda":
             raise RuntimeError(f"model {args.model} needs a CUDA device (hand-written sm_90a kernels)")
         return EngineAdapter(args.model, args.batch, args.seq, args)
@@ -979,7 +977,8 @@ def run(args) -> Dict[str, Any]:
 
 def parse_args(argv=None):
     ap = argparse.ArgumentParser(prog="aitj-worker")
-    ap.add_argument("--model", default="gpt2", choices=["gpt2", "gpt2-tiny", "bert", "bert-tiny", "resnet50", "mnist", "mlp"])
+    ap.add_argument("--model", default="gpt2",
+                    choices=[*GPT2_MODELS, "bert", "bert-tiny", "resnet50", "mnist", "mlp"])
     ap.add_argument("--batch", type=int, default=16, help="per-GPU batch size")
     ap.add_argument("--seq", type=int, default=1024)
     ap.add_argument("--steps", type=int, default=20, help="timed steps (0 = run until SIGTERM)")
@@ -1027,7 +1026,7 @@ def parse_args(argv=None):
                     help="an llm.c gpt2_tokenizer.bin: generations are also reported as text")
     args = ap.parse_args(argv)
     _check_generation_args(ap, args)
-    if args.eval_data and args.model not in ("gpt2", "gpt2-tiny"):
+    if args.eval_data and args.model not in GPT2_MODELS:
         ap.error(f"--eval-data evaluates GPT-2 models only, not {args.model}")
     if args.eval_data and args.gemm != "wgmma":
         ap.error("--eval-data needs --gemm wgmma: the evaluation loss is computed in the wgmma logits GEMM's epilogue")
@@ -1042,12 +1041,10 @@ def parse_args(argv=None):
                  "accumulation")
     if args.doc_mask and not args.data:
         ap.error("--doc-mask needs --data")
-    if args.data and args.model not in ("gpt2", "gpt2-tiny"):
+    if args.data and args.model not in GPT2_MODELS:
         ap.error(f"--data trains GPT-2 models only, not {args.model}")
     if args.data:
-        from ..models.gpt2 import GPT2Config
-
-        vocab = (GPT2Config.small() if args.model == "gpt2" else GPT2Config.tiny()).vocab_size
+        vocab = GPT2_MODELS[args.model].vocab_size
         if args.doc_mask and not 0 <= args.eot_token < vocab:
             ap.error(f"--eot-token {args.eot_token} is outside the vocabulary of {args.model} (size {vocab})")
     return args
@@ -1062,7 +1059,7 @@ def _check_generation_args(ap, args) -> None:
         if given:
             ap.error(f"{', '.join(given)} need --generate-every")
         return
-    if args.model not in ("gpt2", "gpt2-tiny"):
+    if args.model not in GPT2_MODELS:
         ap.error(f"--generate-every generates from GPT-2 models only, not {args.model}")
     args.generate_count = 4 if args.generate_count is None else args.generate_count
     args.generate_tokens = 64 if args.generate_tokens is None else args.generate_tokens
@@ -1072,9 +1069,7 @@ def _check_generation_args(ap, args) -> None:
         ap.error("--generate-every, --generate-tokens, --temperature and --top-k cannot be negative")
     if args.generate_count < 1:
         ap.error(f"--generate-count {args.generate_count}: generate at least one sequence")
-    from ..models.gpt2 import GPT2Config
-
-    cfg = GPT2Config.small() if args.model == "gpt2" else GPT2Config.tiny()
+    cfg = GPT2_MODELS[args.model]
     if args.generate_prompt is None:
         prompt = [args.eot_token]
         what = f"the default prompt, --eot-token {args.eot_token},"
