@@ -10,8 +10,9 @@
 //   `pos` exit at once and a replay stays correct as `pos` grows; at S = 1 the grid still has H x (pos / 64 + 1) CTAs.
 // * embedding_decode: x[s] = wte[tok[s]] + wpe[pos].
 // * sample_tokens: one CTA per sequence over its bf16 logits row (staged in shared memory): greedy argmax, or a draw
-//   from softmax(logits / temperature) restricted to the top_k largest (radix select on the bf16 bits), keyed by a
-//   counter-based Philox of (seed, sequence, pos); prompt positions are forced.  The last CTA to finish moves `pos` on.
+//   from softmax(logits / temperature) restricted to the top_k largest (radix select on the bf16 bits, -0 equal to +0),
+//   keyed by a counter-based Philox of (seed, sequence, pos); prompt positions are forced.  The last CTA to finish moves
+//   `pos` on.
 //
 // The C entry points refuse nothing: ops/functional.py checks every argument before it calls them.
 #include "ptx.cuh"
@@ -169,9 +170,10 @@ __device__ __forceinline__ uint32_t philox_first_word(uint64_t seed, uint32_t se
   return c0;
 }
 
-// order-preserving 16-bit key of a bf16 value: a larger value has a larger key
+// order-preserving 16-bit key of a bf16 value: a larger value has a larger key, and -0 has the key of +0, 0x8000 (they
+// are equal, so a -0 ties with a +0 top_k-th logit and is kept); a negative of magnitude m > 0 has 0x8000 - m
 __device__ __forceinline__ uint32_t bf16_key(uint16_t b) {
-  return (b & 0x8000u) ? (~b & 0xFFFFu) : (b | 0x8000u);
+  return (b & 0x8000u) ? (0x10000u - b) : (b | 0x8000u);
 }
 
 struct SampleArgs {
@@ -200,7 +202,7 @@ __global__ void __launch_bounds__(kSampleThreads) sample_tokens_kernel(SampleArg
   __shared__ float wv[32];
   __shared__ int wi[32];
   __shared__ float wsum[32];
-  __shared__ int sel_token;
+  __shared__ int sel_token, sel_thread;
   __shared__ uint32_t thr_key, k_rem, bin_hi;
   const int s = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int nwarps = kSampleThreads / 32;
@@ -278,7 +280,7 @@ __global__ void __launch_bounds__(kSampleThreads) sample_tokens_kernel(SampleArg
         if (lane >= o) incl += y;
       }
       if (lane == 31) wsum[warp] = incl;
-      if (tid == 0) sel_token = -1;
+      if (tid == 0) sel_thread = -1;
       __syncthreads();
       if (warp == 0) {
         float w = lane < nwarps ? wsum[lane] : 0.f;
@@ -296,20 +298,29 @@ __global__ void __launch_bounds__(kSampleThreads) sample_tokens_kernel(SampleArg
       const uint32_t r = philox_first_word(a.seed, static_cast<uint32_t>(a.first_seq + s), static_cast<uint32_t>(pos));
       float target = static_cast<float>(r >> 8) * (1.0f / 16777216.0f) * total;    // [0, total)
       if (!(target < total)) target = nextafterf(total, 0.f);
-      // the first thread whose inclusive prefix passes the target walks its run
-      if (part > 0.f && excl <= target && target < incl) {
+      // The run holding the target belongs to the last thread with nonzero mass whose exclusive prefix does not pass
+      // it.  The threads' [excl, incl) do not tile [0, total): the tree-ordered sums round differently, so neighbours
+      // can overlap or leave a gap of an ulp, and even taking excl from the predecessor's incl would not do, since the
+      // scan is not monotone (a thread with no mass can end below the one before it).  This rule gives every target
+      // exactly one owner whenever the row has mass: the first thread with mass has excl 0.
+      const unsigned starts = __ballot_sync(0xffffffffu, part > 0.f && excl <= target);
+      if (lane == 0 && starts) atomicMax(&sel_thread, warp * 32 + 31 - __clz(starts));
+      __syncthreads();
+      if (tid == sel_thread) {
+        // a target past the run's rounded sum takes its last column of nonzero probability
         float accp = excl;
         int pick = -1, last = -1;
         for (int c = c0; c < c1; ++c) {
           if (bf16_key(row[c]) < thr) continue;
-          last = c;
-          accp += exp2f((__uint_as_float(static_cast<uint32_t>(row[c]) << 16) - zmax) * scale);
+          const float p = exp2f((__uint_as_float(static_cast<uint32_t>(row[c]) << 16) - zmax) * scale);
+          if (p > 0.f) last = c;
+          accp += p;
           if (target < accp) { pick = c; break; }
         }
         sel_token = pick >= 0 ? pick : last;
       }
       __syncthreads();
-      token = sel_token >= 0 ? sel_token : amax;
+      token = sel_thread >= 0 ? sel_token : amax;
     }
   }
   if (tid == 0) {
