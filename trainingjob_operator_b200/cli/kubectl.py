@@ -581,9 +581,11 @@ class CLI:
 
     def top(self, namespace: str, all_ns: bool) -> int:
         """``kubectl top``'s place in this world: what the jobs' rank-0 workers last reported (``aitj.b200/metrics``,
-        ``aitj.b200/rescale-trace``) -- throughput, step time, world size, in-place recoveries, held-out loss."""
+        ``aitj.b200/rescale-trace``) -- throughput, step time, world size, in-place recoveries, HellaSwag accuracy,
+        held-out loss."""
         jobs = self.cs.elasticdeeplearning_v1().aitrainingjobs("" if all_ns else namespace).list().items
-        rows = [["NAME", "PHASE", "WORLD", "SAMPLES/S", "MS/STEP", "STEPS", "RECOVERIES", "LAST RESCALE", "EVAL LOSS"]]
+        rows = [["NAME", "PHASE", "WORLD", "SAMPLES/S", "MS/STEP", "STEPS", "RECOVERIES", "LAST RESCALE", "HELLASWAG",
+                 "EVAL LOSS"]]
         for j in jobs:
             try:
                 m = json.loads(j.annotations.get("aitj.b200/metrics", "{}")) or {}
@@ -596,6 +598,7 @@ class CLI:
                          f"{m['ms_per_step']:.2f}" if m.get("ms_per_step") else "<none>",
                          str(m.get("steps_done", "<none>")), str(m.get("recoveries", 0)),
                          f"{r['seconds']:.2f}s -> world {r.get('world')}" if r.get("seconds") else "<none>",
+                         f"{m['hellaswag_acc']:.4f}" if m.get("hellaswag_acc") is not None else "<none>",
                          f"{m['eval_loss']:.4f}" if m.get("eval_loss") is not None else "<none>"])
         if len(rows) == 1:
             self.p("No resources found.")

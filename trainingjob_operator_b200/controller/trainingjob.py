@@ -21,6 +21,7 @@ metrics.describe("aitj_rescale_seconds", "membership change observed by the work
                                          "(kind=rescale|recovery)")
 metrics.describe("aitj_job_samples_per_second", "whole-job training throughput reported by rank 0")
 metrics.describe("aitj_job_eval_loss", "mean held-out loss per token of the job's last evaluation, reported by rank 0")
+metrics.describe("aitj_job_hellaswag_acc", "HellaSwag accuracy of the job's last scoring, reported by rank 0")
 metrics.describe("aitj_job_recoveries_total", "in-place recoveries of faultTolerant jobs (a rank was lost, the others kept "
                                               "their state)")
 
@@ -51,6 +52,9 @@ def observe_worker_reports(old: dict, cur: dict) -> None:
             v = rec.get("eval_loss")
             if v is not None:
                 metrics.set_gauge("aitj_job_eval_loss", float(v), labels=labels)
+            v = rec.get("hellaswag_acc")
+            if v is not None:
+                metrics.set_gauge("aitj_job_hellaswag_acc", float(v), labels=labels)
         except (ValueError, TypeError, AttributeError):
             pass
 

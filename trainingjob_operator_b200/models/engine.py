@@ -289,6 +289,16 @@ class TransformerEngine:
             lb.att.view(B, T, H, D).copy_(ot)
             lb.att_in = lb.att
 
+    def _attention_doc_fwd(self, lb: _LayerBufs, doc_start: torch.Tensor):
+        """The wgmma attention forward under the document mask ``doc_start``, whatever ``attn_impl`` training uses
+        (scoring completions packed as documents).  The log-sum-exp buffer is allocated on first use when training runs
+        cuDNN attention."""
+        B, T, H = self.B, self.T, self.cfg.n_head
+        if lb.lse is None:
+            lb.lse = torch.empty(B, H, T, device=self.dev, dtype=torch.float32)
+        self.F.attention_fwd(lb.qkv, lb.att, lb.lse, B, T, H, causal=True, doc_start=doc_start)
+        lb.att_in = lb.att
+
     def _attention_bwd(self, lb: _LayerBufs, d_att: torch.Tensor, d_qkv: torch.Tensor, d_bias: torch.Tensor):
         """d_qkv <- SDPA backward; d_bias (the qkv bias gradient) += colsum(d_qkv), fused into the gather."""
         B, T, H = self.B, self.T, self.cfg.n_head

@@ -110,6 +110,9 @@ class GPT2Engine(TransformerEngine):
         # evaluation (eval_forward): fp64 (sum of NLL, tokens); the cross-entropy partials are allocated on first use
         self.eval_acc = torch.zeros(2, device=self.dev, dtype=torch.float64)
         self._xent_part = self._xent_tgt = None
+        # multiple-choice scoring (score_forward): fp64 (correct, examples); its other buffers are allocated on first use
+        self.choice_acc = torch.zeros(2, device=self.dev, dtype=torch.float64)
+        self._score_bufs = None
 
     def input_tensors(self) -> List[torch.Tensor]:
         """Device tensors a step reads its inputs from, in the order the data source yields them."""
@@ -134,6 +137,12 @@ class GPT2Engine(TransformerEngine):
         if self.backend != "wgmma":
             raise ValueError(f"evaluation needs the wgmma GEMM backend (its fused cross-entropy epilogue), not "
                              f"{self.backend!r}")
+        self._nll_forward(self.eval_acc)
+        return self.eval_acc
+
+    def _nll_forward(self, acc: torch.Tensor, doc_start: torch.Tensor = None) -> None:
+        """The evaluation forward of ``eval_forward`` and ``score_forward``: self.losses <- the per-token NLL of
+        self.tgt, acc += (sum of the NLL, tokens with a target).  ``doc_start``: see ``_trunk``."""
         F, P, cfg = self.F, self.params, self.cfg
         if self._xent_part is None:
             self._xent_part = torch.empty(self.M, F.xent_blocks(cfg.padded_vocab), 2, device=self.dev,
@@ -141,25 +150,65 @@ class GPT2Engine(TransformerEngine):
             self._xent_tgt = torch.empty(self.M, device=self.dev, dtype=torch.float32)
         # a training step captured in a CUDA graph owns the tensors the attention forward leaves behind: keep them
         kept = [(lb.att_in, lb.sdpa_ctx) for lb in self.layers]
-        self._trunk()
+        self._trunk(doc_start)
         for lb, (att_in, ctx) in zip(self.layers, kept):
             lb.att_in, lb.sdpa_ctx = att_in, ctx
         wte = P.w16("wte")
         F.gemm_xent(self.lnf, wte, self.tgt, cfg.vocab_size, self._xent_part, self._xent_tgt,
                     block_n=self._bn(self.M, wte.shape[0], f"fwd:{wte.shape[0]}x{wte.shape[1]}"))
-        F.xent_finish(self._xent_part, self._xent_tgt, self.tgt, self.losses, self.eval_acc)
-        return self.eval_acc
+        F.xent_finish(self._xent_part, self._xent_tgt, self.tgt, self.losses, acc)
 
-    def _trunk(self) -> None:
-        """Embeddings, the layers and the final LayerNorm: self.lnf from self.tok."""
+    @torch.no_grad()
+    def score_forward(self, doc_start: torch.Tensor, spans: torch.Tensor, labels: torch.Tensor, E: int) -> torch.Tensor:
+        """Multiple-choice scoring (HellaSwag) of E examples whose completions are packed as documents into the rows of
+        self.tok / self.tgt (``runtime.hellaswag``): ``doc_start`` (int32 [B*T]) marks the documents, ``spans`` (int32
+        [E, 4, 2], device) holds the (first row, rows) of each completion's targets and ``labels`` (int32 [E], device)
+        the right ending.  The forward of ``eval_forward`` with positions counted from each document's start and the
+        wgmma attention under the document mask -- whatever attention training runs -- then ``choice_score``:
+        ``self.choice_acc`` (fp64 [2], zeroed by the caller) += (correct, examples).  Returns the per-completion mean NLL
+        (fp32 [E, 4]).  Leaves the logits, gradients, optimizer state and ``eval_acc`` as they are."""
+        H = self.cfg.n_head
+        why = [w for bad, w in ((self.backend != "wgmma", f"gemm_backend is {self.backend!r}, not 'wgmma'"),
+                                (not self.causal, "it needs causal attention"),
+                                (self.T % 128, f"the sequence length {self.T} is not a multiple of 128"),
+                                (self.cfg.n_embd // H != 64, f"the head dim {self.cfg.n_embd // H} is not 64")) if bad]
+        if why:
+            raise ValueError("scoring packed completions runs the wgmma GEMMs and document-masked attention, which cannot "
+                             "serve this engine: " + "; ".join(why))
+        if not 1 <= E <= self.M // self.F.CHOICES:
+            raise ValueError(f"E = {E} examples: a micro-batch of {self.M} positions holds 1 to "
+                             f"{self.M // self.F.CHOICES}")
+        if self._score_bufs is None:
+            ds = self.doc_start if self.doc_start is not None else \
+                torch.zeros(self.M, dtype=torch.int32, device=self.dev)
+            self._score_bufs = (ds, torch.zeros(2, dtype=torch.float64, device=self.dev),
+                                torch.empty(self.M // self.F.CHOICES, self.F.CHOICES, dtype=torch.float32,
+                                            device=self.dev))
+        ds, nll_acc, mean = self._score_bufs
+        if doc_start is not ds:
+            ds.copy_(doc_start.reshape(-1), non_blocking=True)
+        # nll_acc only receives xent_finish's (sum of NLL, tokens), which scoring does not use: it is never read or zeroed
+        self._nll_forward(nll_acc, ds)
+        self.F.choice_score(self.losses, spans, labels, mean[:E], self.choice_acc)
+        return mean[:E]
+
+    def _trunk(self, doc_start: torch.Tensor = None) -> None:
+        """Embeddings, the layers and the final LayerNorm: self.lnf from self.tok.  ``doc_start`` (int32 [B*T]): packed
+        documents, each embedded from position 0 and attended to under the document mask by the wgmma kernels."""
         F, P = self.F, self.params
-        F.embedding_fwd(self.tok, P.w16("wte"), P.w16("wpe"), self.x0, self.T)
+        if doc_start is None:
+            F.embedding_fwd(self.tok, P.w16("wte"), P.w16("wpe"), self.x0, self.T)
+        else:
+            F.embedding_doc_fwd(self.tok, P.w16("wte"), P.w16("wpe"), doc_start, self.x0, self.T)
         x = self.x0
         for i, lb in enumerate(self.layers):
             p = f"h{i}."
             self.layernorm_fwd(x, P.w16(p + "ln1_w"), P.w16(p + "ln1_b"), lb.ln1, lb.ln1_mean, lb.ln1_rstd)
             self._linear(lb.ln1, P.w16(p + "qkv_w"), lb.qkv, bias=P.w16(p + "qkv_b"))
-            self._attention_fwd(lb)
+            if doc_start is None:
+                self._attention_fwd(lb)
+            else:
+                self._attention_doc_fwd(lb, doc_start)
             self._linear(lb.att_in, P.w16(p + "proj_w"), lb.res1, bias=P.w16(p + "proj_b"), residual=x)
             self.layernorm_fwd(lb.res1, P.w16(p + "ln2_w"), P.w16(p + "ln2_b"), lb.ln2, lb.ln2_mean, lb.ln2_rstd)
             self._linear(lb.ln2, P.w16(p + "fc_w"), lb.fc_act, bias=P.w16(p + "fc_b"), gelu=True, aux=lb.fc_pre)

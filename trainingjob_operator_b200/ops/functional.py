@@ -587,3 +587,62 @@ def sample_tokens(logits, vocab, tok, out_tokens, prompt, prompt_len, pos, tempe
              out_tokens.data_ptr(), out_tokens.shape[1], prompt.data_ptr(), prompt.shape[1], int(prompt_len),
              pos.data_ptr(), float(temperature), int(top_k), int(seed), int(first_seq), S, _stream())
     return tok
+
+
+# ------------------------------------------------------------------------------------ HellaSwag (ops/csrc/hellaswag.cu)
+# Scoring completions packed as documents into rows (runtime/hellaswag.py).  Like the decode entry points, the library
+# refuses nothing; every argument is checked here.
+CHOICES = 4                  # completions per example
+
+
+def check_embedding_doc_fwd(tok, wte, wpe, doc_start, out, T: int):
+    """(M, C) of a valid ``embedding_doc_fwd`` call; ValueError otherwise."""
+    _tensor(tok, "tok", torch.int64, 1)
+    M = tok.numel()
+    _need(M >= 1, "embedding_doc_fwd needs M >= 1 rows")
+    _tensor(wte, "wte", torch.bfloat16, 2, 16)
+    _tensor(wpe, "wpe", torch.bfloat16, 2, 16)
+    C = wte.shape[1]
+    _need(C % 8 == 0 and wpe.shape[1] == C, f"wte and wpe need the same width, a multiple of 8: {C}, {wpe.shape[1]}")
+    _need(1 <= T <= wpe.shape[0], f"T {T} must be in [1, {wpe.shape[0]}] (the rows of wpe)")
+    _need(M % T == 0, f"M {M} is not a multiple of T {T}")
+    _tensor(doc_start, "doc_start", torch.int32, 1, 8)
+    _need(doc_start.numel() == M, f"doc_start must hold {M} elements, not {doc_start.numel()}")
+    _tensor(out, "out", torch.bfloat16, 2, 16)
+    _need(tuple(out.shape) == (M, C), f"out must be [{M}, {C}], not {tuple(out.shape)}")
+    return M, C
+
+
+def embedding_doc_fwd(tok, wte, wpe, doc_start, out, T: int):
+    """out[r] = wte[tok[r]] + wpe[(r mod T) - doc_start[r]]: ``embedding_fwd`` with positions counted from the first
+    token of each row's document (doc_start int32 [M], as the document-masked attention takes it)."""
+    M, C = check_embedding_doc_fwd(tok, wte, wpe, doc_start, out, T)
+    lib.call("aitj_embedding_doc_fwd", tok.data_ptr(), wte.data_ptr(), wpe.data_ptr(), doc_start.data_ptr(),
+             out.data_ptr(), M, int(T), C, _stream())
+    return out
+
+
+def check_choice_score(loss, spans, labels, mean, acc) -> int:
+    """E of a valid ``choice_score`` call; ValueError otherwise."""
+    _tensor(loss, "loss", torch.float32, 1)
+    _tensor(spans, "spans", torch.int32, 3, 8)
+    E = spans.shape[0]
+    _need(E >= 1, "choice_score needs E >= 1 examples")
+    _need(tuple(spans.shape) == (E, CHOICES, 2), f"spans must be [E, {CHOICES}, 2], not {tuple(spans.shape)}")
+    _tensor(labels, "labels", torch.int32, 1)
+    _need(labels.numel() == E, f"labels must hold {E} elements, not {labels.numel()}")
+    _tensor(mean, "mean", torch.float32, 2)
+    _need(tuple(mean.shape) == (E, CHOICES), f"mean must be [{E}, {CHOICES}], not {tuple(mean.shape)}")
+    _tensor(acc, "acc", torch.float64, 1)
+    _need(acc.numel() == 2, f"acc must hold 2 elements, not {acc.numel()}")
+    return E
+
+
+def choice_score(loss, spans, labels, mean, acc):
+    """mean[e, c] <- the mean of loss[first, first + n) over the span (first, n) = spans[e, c] of each completion (the
+    per-token NLL ``xent_finish`` leaves; every span must lie inside ``loss`` with n >= 1); acc (fp64 [2]) += (examples
+    whose lowest mean -- the first on a tie -- is at labels[e], examples)."""
+    E = check_choice_score(loss, spans, labels, mean, acc)
+    lib.call("aitj_choice_score", loss.data_ptr(), spans.data_ptr(), labels.data_ptr(), E, mean.data_ptr(),
+             acc.data_ptr(), _stream())
+    return mean

@@ -93,6 +93,8 @@ _SIGS = {
     "aitj_attention_decode": [_P, _P, _P, _P, _P, _I, _I, _I, _P],
     "aitj_embedding_decode": [_P, _P, _P, _P, _P, _I, _I, _P],
     "aitj_sample_tokens": [_P, _I, _I, _P, _P, _I, _P, _I, _I, _P, _F, _I, _L, _I, _I, _P],
+    "aitj_embedding_doc_fwd": [_P, _P, _P, _P, _P, _I, _I, _I, _P],
+    "aitj_choice_score": [_P, _P, _P, _I, _P, _P, _P],
 }
 
 

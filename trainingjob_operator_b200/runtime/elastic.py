@@ -186,6 +186,8 @@ class ElasticWatcher:
         keep["recoveries"] = len(result.get("recoveries") or [])
         if result.get("evals"):
             keep.update(eval_loss=result["evals"][-1]["loss"], eval_step=result["evals"][-1]["step"])
+        if result.get("hellaswag"):
+            keep.update(hellaswag_acc=result["hellaswag"][-1]["acc"], hellaswag_step=result["hellaswag"][-1]["step"])
         t = getattr(self, "_live_thread", None)
         if t is not None:
             t.join(5.0)                     # an interim report in flight must not land after (and over) the final one

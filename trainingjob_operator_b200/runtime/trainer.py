@@ -421,5 +421,23 @@ class EngineTrainer:
         total = e.eval_acc.cpu()
         return float(total[0]), int(total[1])
 
+    def score(self, micro_inputs) -> Tuple[int, int]:
+        """Multiple-choice scoring (``engine.score_forward``) of this rank's micro-batches of packed completions,
+        launched eagerly: ``micro_inputs`` yields each one's (tokens, targets, doc_start, spans, labels) in pinned host
+        memory (``runtime.hellaswag.HellaSwagData.inputs``).  The ranks' (correct, examples) are summed by one all-reduce
+        on the job's group, which a rank without micro-batches joins too.  Touches no parameter, gradient or optimizer
+        state."""
+        e = self.engine
+        e.choice_acc.zero_()
+        for tok, tgt, doc_start, spans, labels in micro_inputs:
+            e.tok.copy_(tok, non_blocking=True)
+            e.tgt.copy_(tgt, non_blocking=True)
+            e.score_forward(doc_start, spans.to(e.dev, non_blocking=True), labels.to(e.dev, non_blocking=True),
+                            spans.shape[0])
+        if self.world > 1:
+            dist.all_reduce(e.choice_acc, group=self.group)
+        total = e.choice_acc.cpu()
+        return int(total[0]), int(total[1])
+
     def state_tensors(self) -> List[torch.Tensor]:
         return self.engine.params.state_tensors()

@@ -86,6 +86,11 @@ class EngineAdapter:
                 if self.eval_samples > self.eval_data.n_windows:
                     raise DataError(f"--eval-samples {self.eval_samples}: --eval-data {args.eval_data!r} holds only "
                                     f"{self.eval_data.n_windows} windows of {seq + 1} tokens")
+            if getattr(args, "hellaswag", ""):
+                from .hellaswag import HellaSwagData
+
+                # multiple-choice scoring: the file's completions packed into micro-batches once, pinned
+                self.hellaswag = HellaSwagData(args.hellaswag, cfg.vocab_size, batch, seq, pin=device != "cpu")
             if getattr(args, "generate_every", None) is not None:
                 # text generation at step boundaries: a generator of its own (buffers, KV caches) on the engine's
                 # weights, built at the first generation
@@ -111,6 +116,9 @@ class EngineAdapter:
             self.describe.update(data=args.data, doc_mask=self.engine.doc_mask, windows=self.data.n_windows)
         if hasattr(self, "eval_data"):
             self.describe.update(eval_data=args.eval_data, eval_samples=self.eval_samples)
+        if hasattr(self, "hellaswag"):
+            self.describe.update(hellaswag=args.hellaswag, hellaswag_examples=self.hellaswag.examples,
+                                 hellaswag_micro_batches=self.hellaswag.micro_batches)
 
     def bind(self, group=None, warm_up: bool = False) -> None:
         """(Re-)build the trainer for the current process group; the micro-batch plan follows its world size.
@@ -183,6 +191,21 @@ class EngineAdapter:
         called after each of this rank's micro-batches is enqueued."""
         total, tokens = self.trainer.evaluate(self._eval_inputs(progress))
         return {"loss": total / max(1, tokens), "tokens": tokens, "samples": self.eval_samples}
+
+    def score(self, progress=None) -> Dict[str, Any]:
+        """The job's HellaSwag accuracy (collective: every rank calls it).  ``progress`` is called after each of this
+        rank's micro-batches is enqueued."""
+        hs = self.hellaswag
+
+        def inputs():
+            for k in hs.plan(self.trainer.world, self.trainer.rank):
+                yield hs.inputs(k)
+                heartbeat()
+                if progress is not None:
+                    progress()
+
+        correct, examples = self.trainer.score(inputs())
+        return {"correct": correct, "examples": examples, "acc": correct / max(1, examples)}
 
     def generate(self, step: int, progress=None) -> Dict[str, Any]:
         """``--generate-count`` sequences of the prompt and ``--generate-tokens`` new tokens, sampled with the seed of this
@@ -638,6 +661,10 @@ class _Loop:
         # boundary is generated once per process whatever happens to the group around it
         self.generations: List[Dict[str, Any]] = []
         self.last_generate_step = -1
+        # HellaSwag (--hellaswag): at the same boundaries, after the evaluation and before the generation; collective,
+        # so a (re-)bind forgets which boundary was scored, exactly as for the evaluation
+        self.hellaswag: List[Dict[str, Any]] = []
+        self.last_hellaswag_step = -1
 
     def _join_job(self) -> None:
         """Join the job's process group and take its state, and with it the loop step to start at."""
@@ -714,7 +741,7 @@ class _Loop:
             self.breaker.tripped = False
             self.breaker.progress(self.generation)
         self.adapter.bind(None)
-        self.last_eval_step = -1
+        self.last_eval_step = self.last_hellaswag_step = -1
         try:
             with guarded(self.breaker, "the state hand-off", self.generation):
                 self.step = sync_state(self.adapter, self.step, self.device)
@@ -804,6 +831,20 @@ class _Loop:
         self.live_eval_s += wall_ms / 1e3
         return out, ms
 
+    def _hellaswag_due(self) -> bool:
+        s, a = self.step, self.args
+        return hasattr(self.adapter, "hellaswag") and s != self.last_hellaswag_step and \
+            ((s > 0 and a.hellaswag_every > 0 and s % a.hellaswag_every == 0) or (a.steps > 0 and s >= self.total))
+
+    def _score(self) -> None:
+        rec, ms = self._off_the_clock("a HellaSwag scoring", lambda progress: self.adapter.score(progress=progress))
+        rec = dict(step=self.step, **rec, ms=round(ms, 3))
+        self.hellaswag.append(rec)
+        self.last_hellaswag_step = self.step
+        if self.rank == 0:
+            self._log(f"step {self.step}: hellaswag acc {rec['acc']:.4f} ({rec['correct']}/{rec['examples']}) in "
+                      f"{ms:.1f} ms")
+
     def _generate_due(self) -> bool:
         s, a = self.step, self.args
         every = getattr(a, "generate_every", None)
@@ -833,7 +874,8 @@ class _Loop:
                       f"({rec['tokens']} tokens) in {ms:.1f} ms")
 
     def run(self) -> Dict[str, Any]:
-        while (self.step < self.total or self._eval_due() or self._generate_due()) and not self.stopping:
+        while (self.step < self.total or self._eval_due() or self._hellaswag_due() or self._generate_due()) and \
+                not self.stopping:
             if self.breaker is not None:
                 self.breaker.progress(self.generation)
                 # patience from this generation's completed steps: the first step on a freshly bound trainer captures
@@ -847,6 +889,8 @@ class _Loop:
                     self.region.arm(self.step, self.world)
                 if self._eval_due():
                     self._evaluate()
+                if self._hellaswag_due():
+                    self._score()
                 if self._generate_due():
                     self._generate()
                 if self.step >= self.total:
@@ -914,6 +958,8 @@ class _Loop:
                     "steps_done": self.step, "global_batch": G, "recoveries": len(self.recoveries)}
             if self.evals:
                 live.update(eval_loss=self.evals[-1]["loss"], eval_step=self.evals[-1]["step"])
+            if self.hellaswag:
+                live.update(hellaswag_acc=self.hellaswag[-1]["acc"], hellaswag_step=self.hellaswag[-1]["step"])
             self.watcher.report_live(self.rank, live)
         self.live_t0, self.live_step0, self.live_eval_s = time.time(), self.step, 0.0
 
@@ -926,6 +972,9 @@ class _Loop:
             result["data_position"] = adapter.data_position
         if hasattr(adapter, "eval_data"):
             result.update(evals=self.evals, eval_loss_last=self.evals[-1]["loss"] if self.evals else None)
+        if hasattr(adapter, "hellaswag"):
+            result.update(hellaswag=self.hellaswag,
+                          hellaswag_acc_last=self.hellaswag[-1]["acc"] if self.hellaswag else None)
         if hasattr(adapter, "generator"):
             result["generations"] = self.generations
         if self.breaker is not None:
@@ -1012,6 +1061,12 @@ def parse_args(argv=None):
     ap.add_argument("--eval-every", type=int, default=0, metavar="N",
                     help="evaluate before every step that is a multiple of N, and after the last step (0 = only after "
                          "the last step)")
+    ap.add_argument("--hellaswag", default="", metavar="PATH",
+                    help="score HellaSwag from this llm.c eval file (dev/data/hellaswag.py; GPT-2 models, wgmma GEMMs, "
+                         "--seq a multiple of 128)")
+    ap.add_argument("--hellaswag-every", type=int, default=None, metavar="N",
+                    help="score HellaSwag before every step that is a multiple of N, and after the last step (0 = only "
+                         "after the last step)")
     # text generation (GPT-2): "generate", because "samples" already names data windows here
     ap.add_argument("--generate-every", type=int, default=None, metavar="N",
                     help="generate text before every step that is a multiple of N, and after the last step (0 = only "
@@ -1034,6 +1089,7 @@ def parse_args(argv=None):
         ap.error("--eval-samples and --eval-every cannot be negative")
     if (args.eval_samples or args.eval_every) and not args.eval_data:
         ap.error("--eval-samples and --eval-every need --eval-data")
+    _check_hellaswag_args(ap, args)
     if args.global_batch < 0 or args.global_batch % args.batch:
         ap.error(f"--global-batch {args.global_batch} is not a multiple of --batch {args.batch}")
     if args.global_batch and os.environ.get("AITJ_ALLREDUCE") == "mc":
@@ -1048,6 +1104,23 @@ def parse_args(argv=None):
         if args.doc_mask and not 0 <= args.eot_token < vocab:
             ap.error(f"--eot-token {args.eot_token} is outside the vocabulary of {args.model} (size {vocab})")
     return args
+
+
+def _check_hellaswag_args(ap, args) -> None:
+    if args.hellaswag_every is not None and not args.hellaswag:
+        ap.error("--hellaswag-every needs --hellaswag")
+    args.hellaswag_every = args.hellaswag_every or 0
+    if not args.hellaswag:
+        return
+    if args.model not in GPT2_MODELS:
+        ap.error(f"--hellaswag scores GPT-2 models only, not {args.model}")
+    if args.gemm != "wgmma":
+        ap.error("--hellaswag needs --gemm wgmma: the completions' losses are computed in the wgmma logits GEMM's "
+                 "epilogue")
+    if args.seq % 128:
+        ap.error(f"--hellaswag needs --seq a multiple of 128 (the document-masked attention's tile), not {args.seq}")
+    if args.hellaswag_every < 0:
+        ap.error("--hellaswag-every cannot be negative")
 
 
 def _check_generation_args(ap, args) -> None:
